@@ -1,4 +1,4 @@
-"""bazuka_b200 — B200-native kernels for Bazuka's MPN Groth16 proving path.
+"""bazuka_b200 — H100-native kernels for Bazuka's MPN Groth16 proving path.
 
 Host-side mirror of the reference's interfaces for this path, over libbzk's C ABI:
 

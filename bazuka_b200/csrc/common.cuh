@@ -11,7 +11,7 @@
 
 namespace bzk {
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM; bzk_ctx_create replaces it with the device's count
 
 struct PoseidonTable {
     uint32_t t = 0, rf = 0, rp = 0, nrc = 0;

@@ -5,7 +5,7 @@
 //  `(Fp,Fp,bool)` / `((Fp,Fp),(Fp,Fp),bool)`, /root/reference/src/zk/groth16/mod.rs:21-38, and through
 //  bellman's multiexp inside create_proof, call sites /root/reference/src/mpn/circuits/test.rs:135,175,215).
 //
-// Representation choices (B200-first, not the crate's):
+// Representation choices (GPU-first, not the crate's):
 //   * bases in HBM:  packed affine {x,y}, 96 B (G1) / 192 B (G2), 16-byte aligned so a point is
 //     6 / 12 LDG.128;  identity is encoded as x = y = 0 (not on the curve, b != 0).  The 104 / 200-byte
 //     crate images (x | y | infinity byte | pad) are converted at the C-ABI boundary.

@@ -1,4 +1,4 @@
-// bazuka_b200 — Montgomery prime-field arithmetic for sm_100a (and a bit-identical host path).
+// bazuka_b200 — Montgomery prime-field arithmetic for sm_90a (and a bit-identical host path).
 //
 // Replaces, on the GPU, what the reference obtains from un-vendored crates:
 //   Fr  = `ZkScalar([u64;4])`            /root/reference/src/zk/mod.rs:202-206   (ff 0.13 derive)
@@ -6,7 +6,7 @@
 // Memory image = the reference's: little-endian 64-bit limbs in Montgomery form (R = 2^256 / 2^384),
 // always fully reduced, so device results can be memcmp'd against the CPU prover's.
 //
-// Blackwell has no 64-bit integer multiplier; the native wide op is IMAD.WIDE.U32 (32x32+64 with
+// Hopper has no 64-bit integer multiplier; the native wide op is IMAD.WIDE.U32 (32x32+64 with
 // carry-in/out predicates).  The product is therefore organised on 32-bit limbs as two interleaved
 // accumulators — one holding the 64-bit partial products that start on even columns, one those
 // that start on odd columns — so that every 32x32 product is ONE `mad.lo.cc/madc.hi.cc` pair
@@ -58,14 +58,9 @@ BZK_D uint32_t mul_lo(uint32_t a, uint32_t b) { return a * b; }
 BZK_D uint32_t mul_hi(uint32_t a, uint32_t b) { return __umulhi(a, b); }
 // (hi:lo) += a*b with the carry chained through, as ONE asm statement so that ptxas emits a single
 // IMAD.WIDE.U32.X per product (as separate statements it splits register-register products into
-// IMAD + IMAD.HI + 2 IADD3.X).  Measured on B200 (tools/microbench/imad.cu, profiles/): IMAD,
-// IMAD.HI and carry-less IMAD.WIDE each hold the fmaheavy pipe 2 cycles per warp, IMAD.WIDE.U32.X
-// ~4.4 and a carry-in/carry-out IADD3.X ~3.2 on the ALU pipe.  Per 384-bit product that is
-//   fused (this)              301 heavy instr                    -> 1276 cycles/warp   <- used
-//   IMAD+IMAD.HI+2 IADD3.X    433 heavy + 295 IADD3.X            -> 1240
-//   IMAD.WIDE + 2 IADD3.X     310 heavy + 575 IADD3.X            -> 1864
-// i.e. carries, not multiplies, are what is expensive on this part; the carry-free way out
-// (unsaturated 28/30-bit limbs, plain IMAD.WIDE only) is the round-2 multiplier.
+// IMAD + IMAD.HI + 2 IADD3.X).  Per 384-bit product that is 301 heavy instructions fused (this),
+// 433 heavy + 295 IADD3.X split, or 310 heavy + 575 IADD3.X with carry-less IMAD.WIDE: carries,
+// not multiplies, dominate the instruction count.  tools/microbench/imad.cu times the three forms.
 #ifndef BZK_MUL_WIDE_ADD
 BZK_D void mad_pair_first(uint32_t &lo, uint32_t &hi, uint32_t a, uint32_t b, CC &) {
     BZK_ASM("mad.lo.cc.u32 %0,%2,%3,%0; madc.hi.cc.u32 %1,%2,%3,%1;" : "+r"(lo), "+r"(hi) : "r"(a), "r"(b));

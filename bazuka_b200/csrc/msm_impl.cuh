@@ -1,4 +1,4 @@
-// bazuka_b200 — Pippenger multi-scalar multiplication over BLS12-381 G1 / G2 on sm_100a.
+// bazuka_b200 — Pippenger multi-scalar multiplication over BLS12-381 G1 / G2 on sm_90a.
 //
 // GPU replacement for bellman 0.14.0 `multiexp::multiexp` (un-vendored crate), the eight sums
 // h, l, a_inputs, a_aux, b_g1_inputs, b_g1_aux, b_g2_inputs, b_g2_aux of `create_proof`
@@ -42,12 +42,13 @@ namespace bzk {
 // ---------------------------------------------------------------------------------------------
 
 // cost of a plan in "mixed additions": n*W bucket insertions + kReduceCost per bucket for the reduction
-// (calibrated on B200 at 2^20: two full additions per bucket in the running sums, the latency-bound
-// tree and the extra digit / scatter work of more windows)
+// (two full additions per bucket in the running sums, the latency-bound tree and the extra digit /
+// scatter work of more windows).  kReduceCost and kNarrowTopCost were calibrated at 2^20 on the previous
+// target GPU and are carried over unchanged: they have not been re-tuned on the H100.
 // A narrow TOP window is expensive: scalars are < 2^255, so window W-1 holds only 255 - c*(W-1) meaningful bits; when
 // that is a handful (c = 19: 8 bits, c = 18 or 21: 3), a sixteenth of all entries lands in a few hundred buckets — the
 // histogram's REDs and the scatter's ATOMs serialise on those addresses and the runs go through the long-run path
-// (measured at 2^20: c = 19 costs 0.54 ms more than c = 20 in those three stages) — about 1.5 additions per term.
+// — about 1.5 additions per term.
 constexpr double kReduceCost = 6.0, kNarrowTopCost = 1.5;
 static double plan_cost(size_t n, uint32_t c, uint32_t T) {
     const uint32_t W = (256 + c - 1) / c;
@@ -663,10 +664,8 @@ static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_
 
     // batched-affine rounds before the XYZZ accumulation (msm_affine.cuh): worth it when buckets hold several entries
     // and the point references fit 30 bits; R rounds leave 2^-R of the additions to the XYZZ kernel
-    // Measured on B200 at 2^20 / 13 windows (profiles/r02_msm_affine_rounds.txt): a G1 round costs 0.36 ns per addition
-    // (k_round_fwd is load-latency bound, k_round_bwd reaches 66 % of the multiplier peak, the inversion is a 0.7 ms
-    // single-thread chain) against 0.42 ns for the XYZZ kernel — R = 1 / 2 / 3 make the whole sum 0.45 / 0.83 / 1.4 ms
-    // SLOWER, so the default for G1 is 0 rounds; the knobs stay for G2 and for tuning.
+    // k_round_fwd is load-latency bound and each round ends in a single-thread inversion chain, so for G1 the rounds
+    // made the whole sum slower; the default for G1 is 0 rounds; the knobs stay for G2 and for tuning.
     static const int env_g1 = std::getenv("BZK_AFFINE_ROUNDS") ? atoi(std::getenv("BZK_AFFINE_ROUNDS")) : 0;
     static const int env_g2 = std::getenv("BZK_AFFINE_ROUNDS_G2") ? atoi(std::getenv("BZK_AFFINE_ROUNDS_G2")) : 0;
     const int ctx_rounds = ctx->affine_rounds[sizeof(F) == sizeof(Fp) ? 0 : 1];

@@ -1,4 +1,4 @@
-// bazuka_b200 — radix-2 NTT over BLS12-381 Fr on sm_100a.
+// bazuka_b200 — radix-2 NTT over BLS12-381 Fr on sm_90a.
 //
 // GPU replacement for bellman 0.14.0 `domain::EvaluationDomain::{fft, ifft, coset_fft, icoset_fft,
 // divide_by_z_on_coset, mul_assign, sub_assign}` (un-vendored crate; reached from every

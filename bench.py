@@ -4,6 +4,9 @@ of the headline metric "MPN Groth16 proofs/sec ...; G1 MSM scalars/sec vs HBM ro
 
   python bench.py --gpus N --steps K --warmup W            our arm  (N>1: launched under torchrun)
   python bench.py --impl reference --gpus N --steps K ...   the CPU arm (rank 0 only)
+  --dump-outputs DIR   after the timed steps, rank 0 writes the MSM sum of the last timed step as
+                       DIR/g1_msm_sum.npy (its 104-byte affine image, one float32 per byte); the inputs
+                       are seeded, so two builds can be compared output for output
 
 A step = one multi-scalar multiplication sum_i [s_i] P_i over synthetic inputs: per GPU 2^20
 uniform Fr scalars (SplitMix64) and 2^20 bases P_i = [k_i] G.  At N GPUs the job is ONE MSM of
@@ -49,7 +52,7 @@ class ClockSampler:
     """nvidia-smi clocks / throttle reasons sampled every 200 ms during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit,name")
 
     def __init__(self, gpu_index):
         self.idx = gpu_index
@@ -83,8 +86,9 @@ class ClockSampler:
         mx = [int(r[2]) for r in self.rows if len(r) >= 8 and r[2].isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = sorted({names[k] for r in self.rows if len(r) >= 8 for k in range(4) if r[4 + k].lower().startswith("active")})
-        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None,
-                "reasons": reasons, "samples": len(self.rows)}
+        last = self.rows[-1] if self.rows and len(self.rows[-1]) >= 10 else [None] * 10
+        return {"gpu": last[9], "power_limit_w": last[8], "sm_mhz": sm[len(sm) // 2] if sm else None,
+                "sm_max_mhz": max(mx) if mx else None, "reasons": reasons, "samples": len(self.rows)}
 
 
 def measured_peak():
@@ -94,18 +98,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic():
-    """dram bytes per launch of the dominant kernel from the committed ncu --set full capture."""
-    p = os.path.join(ROOT, "profiles", "msm_accumulate_ncu.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get("dram_bytes_per_launch")
-        except Exception:
-            return None
-    return None
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -192,7 +185,7 @@ def run_ours(args, rank, local_rank, world):
     ctx.fr_random_dev(rank_inputs_seeds(rank)[1], n, d_scalars)
     h_scalars = d_scalars.cpu().pin_memory()
     h_img = d_img.cpu().pin_memory() if rank == 0 else None
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(512 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
     torch.cuda.synchronize()
 
     from bazuka_b200 import dist as bd
@@ -246,6 +239,9 @@ def run_ours(args, rank, local_rank, world):
 
     total_ms, wall, result = timed(step_resident, args.steps, args.warmup, begin_region)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "g1_msm_sum.npy"), np.asarray(result, dtype=np.uint8).astype(np.float32))
     launches = ctx.launch_count - launches[0]
     runs, _, stage_sum = ctx.stage_ms()
     ctx.set_timing(False)
@@ -263,7 +259,7 @@ def run_ours(args, rank, local_rank, world):
     if not args.no_mpn:
         # the proofs/s half of the metric on a whole update batch (all ranks: the N>1 schedules have collectives)
         from tools.mpn_batch_bench import batch_section
-        shape = (16, 3, 5) if args.workload == "mpn1024" else (15, 3, 4)
+        shape = (16, 3, 4) if args.workload == "depth32" else (15, 3, 4)
         try:
             batch = batch_section(ctx, *shape, steps=args.mpn_steps, dist=dist, rank=rank, world=world, peak_gbs=measured_peak()[0])
         except Exception as e:
@@ -286,7 +282,7 @@ def run_ours(args, rank, local_rank, world):
         "config": {
             "workload": workload_string(args.log_n, world),
             "terms_total": world * n, "parallelism": f"base-sharded x{world}, 1 NCCL all-gather of {104 * world} B" if world > 1 else "single GPU",
-            "l2": "512 MiB write before every timed step (L2 flushed); inputs 132 MB > 126 MB L2",
+            "l2": "512 MiB write before every timed step (L2 flushed); inputs 132 MB > 50 MB L2",
             "timing": "CUDA events on the launching stream per step, barrier+sync around region, max over ranks",
             "result_check": "sum folded on every rank; e2e result == resident result",
             "bases": f"resident with a fixed-base table of {table_levels} levels ({96 * table_levels * n >> 20} MiB per GPU, built once in "
@@ -298,9 +294,9 @@ def run_ours(args, rank, local_rank, world):
         "roofline": {
             "bound": "hbm", "kernel": "k_accumulate<Fp> (bucket accumulation, mixed XYZZ adds)",
             "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": (achieved / peak) if achieved else None,
-            "traffic": ncu_traffic(), "peak_source": peak_src,
+            "peak_source": peak_src,
             "algorithmic_bytes_per_launch": ALGO_BYTES_PER_TERM * n,
-            "kernel_ms": acc_ms, "frac_of_nominal_8TBs": (achieved / 8000.0) if achieved else None,
+            "kernel_ms": acc_ms, "frac_of_nominal_3_35TBs": (achieved / 3350.0) if achieved else None,
             "note": "integer-ALU bound (13 windows over the fixed-base table x ~11 Fp products per term); see DESIGN.md section 3.1-3.2 for the IMAD roofline",
         },
         "e2e": {"value": world * n / (e2e_step * 1e-3), "unit": UNIT, "ms_per_step": e2e_step,
@@ -486,9 +482,11 @@ def main():
     ap.add_argument("--log-n", type=int, default=LOG_N_DEFAULT)
     ap.add_argument("--table-levels", type=int, default=16, help="fixed-base table levels for the resident bases (1 = none)")
     ap.add_argument("--no-mpn", action="store_true", help="skip the MPN proof sections (single update + whole update batch)")
-    ap.add_argument("--workload", default="mpn256", choices=["mpn256", "mpn1024"],
-                    help="update batch proved in the mpn_groth16 section: production 256-tx batch (2^24) or BASELINE configs[3] 1024-tx (2^26)")
+    ap.add_argument("--workload", default="mpn256", choices=["mpn256", "depth32"],
+                    help="update batch proved in the mpn_groth16 section: production 256-tx batch (2^24) or BASELINE configs[3]'s "
+                         "depth-32 tree at 256 tx (A=16, 2^24); its 1024-tx batch (2^26) does not fit one 80 GB H100")
     ap.add_argument("--mpn-steps", type=int, default=3, help="timed update-batch proofs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's MSM sum to DIR/g1_msm_sum.npy")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

@@ -1,4 +1,4 @@
-/* libbzk — B200-native prover kernels for Bazuka's MPN Groth16 path.  C ABI (drop-in boundary).
+/* libbzk — H100-native prover kernels for Bazuka's MPN Groth16 path.  C ABI (drop-in boundary).
  *
  * Everything here is plain C: opaque handles, raw pointers and sizes, int32 status codes.  No
  * exception, abort or global mutable state crosses this boundary.  One `bzk_ctx` per GPU; calls

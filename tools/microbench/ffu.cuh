@@ -1,8 +1,8 @@
-// bazuka_b200 — carry-free ("unsaturated limb") Fp for the MSM inner loops on sm_100a.
+// bazuka_b200 — carry-free ("unsaturated limb") Fp for the MSM inner loops on sm_90a.
 //
-// Why: on B200 every IMAD-class instruction occupies the fmaheavy pipe for 2 cycles per warp except
-// the carry forms (IMAD.WIDE.U32.X ~4.4, carry-in/out IADD3.X ~3.2 on the ALU pipe) — see
-// profiles/r01_microbench_int_pipes.txt and the table in ff.cuh.  A saturated 12 x 32-bit Montgomery
+// Why: the carry forms of the integer multiply (IMAD.WIDE.U32.X, carry-in/out IADD3.X) cost more
+// issue slots than plain IMAD-class instructions — imad.cu times them, ff.cuh counts them per
+// product.  A saturated 12 x 32-bit Montgomery
 // product needs a carry on every one of its 288 partial products.  With 13 limbs of 30 bits the
 // partial products are < 2^60, so a 64-bit column accumulator absorbs 14 of them without any carry:
 // the product becomes 338 plain IMAD.WIDE.U32 (t[j] += a[j]*b[i]) + 13 IMAD, carries are handled by

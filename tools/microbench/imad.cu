@@ -1,4 +1,4 @@
-// Integer-pipe microbenchmark for sm_100a: what does a 32x32 multiply cost in each SASS form?
+// Integer-pipe microbenchmark for sm_90a: what does a 32x32 multiply cost in each SASS form?
 // Prints warp-instructions per clock per SM for independent chains of each op.
 #include <cstdio>
 #include <cstdint>

@@ -2,8 +2,9 @@
 
     bzk_mpn_update_build  ->  bzk_mpn_update_witness  ->  bzk_groth16_prove_dev        (include/bzk.h)
 
-for the production batch (A=15, T=3, B=4: 256 transfers, 14.4 M constraints, 2^24 domain;
-/root/reference/src/config/blockchain.rs:22-26) or BASELINE configs[3] (A=16, B=5: 1024 transfers, 2^26).
+for the production batch (A=15, T=3, B=4: 256 transfers, 14.4 M constraints, 2^24 domain; the reference's
+src/config/blockchain.rs:22-26) or BASELINE configs[3]'s depth-32 tree at the same batch (A=16, B=4, 2^24).  The 1024-transfer
+batch of configs[3] (B=5, 2^26) does not fit the 80 GB of one H100.
 Called by bench.py (default run: production batch at N=1; under torchrun also the (R) replicas and (S) base-sharded
 schedules of SURVEY.md §8e) and usable stand-alone:
 
