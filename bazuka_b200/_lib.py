@@ -39,6 +39,8 @@ SIGNATURES = {
     "bzk_ctx_launch_count": (_u64, [_vp]),
     "bzk_ctx_set_timing": (_i32, [_vp, _i32]),
     "bzk_ctx_set_msm_affine_rounds": (_i32, [_vp, _i32, _i32]),
+    "bzk_ctx_set_msm_table_window": (_i32, [_vp, _u32]),
+    "bzk_ctx_last_msm_plan": (_i32, [_vp, _vp]),
     "bzk_ctx_stage_ms": (_u64, [_vp, _vp, _vp, _u32]),
     "bzk_poseidon_load_params": (_i32, [_vp, _vp, _sz]),
     "bzk_poseidon_hash": (_i32, [_vp, _u32, _vp, _sz, _vp]),

@@ -139,6 +139,19 @@ class Context:
         """batched-affine rounds before the XYZZ accumulation (speed knob; results unchanged); -1 = library default"""
         self._check(self._l.bzk_ctx_set_msm_affine_rounds(self._h, int(g1), int(g2)))
 
+    def set_msm_table_window(self, c=0):
+        """window of the fixed-base tables built from now on (8..23); 0 = the planner's choice.  Results unchanged."""
+        self._check(self._l.bzk_ctx_set_msm_table_window(self._h, int(c)))
+
+    MSM_PLAN_FIELDS = ("c", "W", "T", "G", "NB", "slice", "nbits", "long_len")
+
+    def last_msm_plan(self):
+        """plan of the last single MSM on this context (bzk_ctx_last_msm_plan) as a dict of MSM_PLAN_FIELDS;
+        long_len is only read back while set_timing(True) is on."""
+        out = np.zeros(8, dtype=np.uint32)
+        self._check(self._l.bzk_ctx_last_msm_plan(self._h, _host_ptr(out)))
+        return dict(zip(self.MSM_PLAN_FIELDS, (int(x) for x in out)))
+
     def stage_ms(self):
         """-> (runs, last_ms[16], sum_ms[16]) from the CUDA events the MSM driver records between kernels."""
         last = np.zeros(16, dtype=np.float32)

@@ -106,7 +106,7 @@ const char *bzk_strerror(int32_t s) {
     }
 }
 const char *bzk_last_error(const bzk_ctx *ctx) { return ctx ? ctx->err : "null ctx"; }
-uint32_t bzk_abi_version(void) { return (1u << 16) | 0u; }
+uint32_t bzk_abi_version(void) { return (1u << 16) | 1u; }
 
 int32_t bzk_ctx_create(int32_t device, bzk_ctx **out) {
     if (!out) return BZK_ERR_BAD_ARG;
@@ -169,6 +169,16 @@ int32_t bzk_ctx_set_msm_affine_rounds(bzk_ctx *ctx, int32_t g1_rounds, int32_t g
     if (!ctx || g1_rounds > 6 || g2_rounds > 6) return BZK_ERR_BAD_ARG;
     ctx->affine_rounds[0] = g1_rounds;
     ctx->affine_rounds[1] = g2_rounds;
+    return BZK_OK;
+}
+int32_t bzk_ctx_set_msm_table_window(bzk_ctx *ctx, uint32_t c) {
+    if (!ctx || (c != 0 && (c < 8 || c > 23))) return BZK_ERR_BAD_ARG;
+    ctx->table_c = c;
+    return BZK_OK;
+}
+int32_t bzk_ctx_last_msm_plan(const bzk_ctx *ctx, uint32_t out[8]) {
+    if (!ctx || !out) return BZK_ERR_BAD_ARG;
+    memcpy(out, ctx->last_plan, sizeof ctx->last_plan);
     return BZK_OK;
 }
 uint64_t bzk_ctx_stage_ms(const bzk_ctx *ctx, float *last_ms, double *sum_ms, uint32_t cap) {

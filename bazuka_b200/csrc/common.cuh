@@ -57,6 +57,9 @@ struct bzk_ctx {
     bzk::Fr *d_gpow = nullptr;  // coset generator power tables, see ntt.cu
     int sm_count = bzk::kNumSMs;
     int affine_rounds[2] = {-1, -1};  // batched-affine rounds for G1 / G2 sums (-1: BZK_AFFINE_ROUNDS[_G2] or the default 0)
+    uint32_t table_c = 0;             // window of the fixed-base tables built from now on (0: BZK_TABLE_C or the cost model)
+    // plan of the last single MSM (msm_run): c, W, T, G, NB, slice, nbits, long-run queue length (timing on, else 0)
+    uint32_t last_plan[8] = {0};
     // side streams + arenas so that independent MSMs of one proof run concurrently (groth16.cu)
     cudaStream_t aux_stream[4] = {nullptr, nullptr, nullptr, nullptr};
     void *aux_ws[4] = {nullptr, nullptr, nullptr, nullptr};

@@ -78,11 +78,13 @@ static MsmPlan make_plan(size_t n, uint32_t c_tab = 0, uint32_t T = 1, uint32_t 
     p.TB = p.G * p.NB;
     return p;
 }
-// window size and level count of the table to build for an n-point resident vector
-static void choose_table(size_t n, uint32_t max_levels, uint32_t *c_out, uint32_t *T_out, uint32_t *G_out) {
+// window size and level count of the table to build for an n-point resident vector; ctx_c != 0 forces the window
+// (bzk_ctx_set_msm_table_window), else the BZK_TABLE_C environment value does, else the cost model picks it
+static void choose_table(size_t n, uint32_t max_levels, uint32_t ctx_c, uint32_t *c_out, uint32_t *T_out, uint32_t *G_out) {
     double best = 1e300;
     uint32_t bc = 16, bT = 1;
-    static const uint32_t force_c = std::getenv("BZK_TABLE_C") ? (uint32_t)atoi(std::getenv("BZK_TABLE_C")) : 0;  // tuning aid
+    static const uint32_t env_c = std::getenv("BZK_TABLE_C") ? (uint32_t)atoi(std::getenv("BZK_TABLE_C")) : 0;  // tuning aid
+    const uint32_t force_c = ctx_c ? ctx_c : env_c;
     for (uint32_t c = 8; c <= 23; c++) {
         if (force_c && c != force_c) continue;
         const uint32_t W = (256 + c - 1) / c;
@@ -620,7 +622,7 @@ static int32_t bases_precompute(bzk_ctx *ctx, Affine<F> **d, size_t n, uint32_t 
     if (max_levels > kMaxLevels) max_levels = kMaxLevels;
     uint32_t c = 0, T = 1, G = 0;
     if (n == 0 || max_levels <= 1) { *c_out = 0; *T_out = 1; *G_out = 0; return BZK_OK; }
-    choose_table(n, max_levels, &c, &T, &G);
+    choose_table(n, max_levels, ctx->table_c, &c, &T, &G);
     if (T <= 1) { *c_out = 0; *T_out = 1; *G_out = 0; return BZK_OK; }
     Affine<F> *tab = nullptr;
     cudaError_t e = cudaMalloc(&tab, (size_t)T * n * sizeof(Affine<F>));
@@ -643,8 +645,9 @@ template <class F>
 // `h_win` (host, ideally pinned; >= 64 entries) by the last operation on the stream.  Nothing here
 // synchronises: several MSMs can be in flight on different streams (the Groth16 driver runs its
 // five sums concurrently), and msm_host_finish folds the window sums once the stream is done.
+// `d_long_len` (optional) receives the device address of the long-run queue length k_fixup counts.
 static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, bool timed, const BasesRef<F> &bases,
-                           const Fr *d_scalars, size_t n, Xyzz<F> *h_win, MsmPlan *plan_out) {
+                           const Fr *d_scalars, size_t n, Xyzz<F> *h_win, MsmPlan *plan_out, uint32_t **d_long_len = nullptr) {
     if (n == 0) { plan_out->W = 0; return BZK_OK; }
     if (n >= ((size_t)1 << 31) || bases.off + n > bases.n_tab) return BZK_ERR_BAD_ARG;
     const MsmPlan pl = make_plan(n, bases.c, bases.T, bases.G);
@@ -756,6 +759,7 @@ static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_
     int32_t *part_bucket = cv.take<int32_t>(nslots);
     LongRun *long_queue = cv.take<LongRun>(kLongQueueCap);
     uint32_t *long_len = cv.take<uint32_t>(4);
+    if (d_long_len) *d_long_len = long_len;
     Xyzz<F> *slice_acc = cv.take<Xyzz<F>>(nslices), *slice_run = cv.take<Xyzz<F>>(nslices);
     Xyzz<F> *partial = cv.take<Xyzz<F>>((size_t)rows * parts);
     Xyzz<F> *win_out = cv.take<Xyzz<F>>(rows);
@@ -878,9 +882,15 @@ static int32_t msm_run(bzk_ctx *ctx, const BasesRef<F> &d_bases, const Fr *d_sca
     static_assert(kMaxWinPoints * sizeof(Xyzz<F>) <= 160 * 1024, "h_win on the stack");
     Xyzz<F> h_win[kMaxWinPoints];
     MsmPlan pl;
-    BZK_TRY(msm_enqueue<F>(ctx, ctx->stream, &ctx->ws, &ctx->ws_bytes, true, d_bases, d_scalars, n, h_win, &pl));
+    uint32_t *d_long_len = nullptr;
+    BZK_TRY(msm_enqueue<F>(ctx, ctx->stream, &ctx->ws, &ctx->ws_bytes, true, d_bases, d_scalars, n, h_win, &pl, &d_long_len));
+    // the plan this call ran (bzk_ctx_last_msm_plan); the queue length costs a copy, so only with timing on
+    uint32_t long_len = 0;
+    if (ctx->timing && d_long_len) BZK_CUDA(ctx, cudaMemcpyAsync(&long_len, d_long_len, sizeof long_len, cudaMemcpyDeviceToHost, ctx->stream));
     BZK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     timing_collect(ctx);
+    const uint32_t rec[8] = {pl.c, pl.W, pl.T, pl.G, pl.NB, pl.slice, pl.nbits, long_len};
+    memcpy(ctx->last_plan, rec, sizeof rec);
     msm_host_finish<F>(pl, h_win, out);
     return BZK_OK;
 }

@@ -110,25 +110,29 @@ class ProvingKey:
             pass
 
 
-def proving_key_from_host(ctx, vk, h, l, a, b_g1, b_g2):
+def proving_key_from_host(ctx, vk, h, l, a, b_g1, b_g2, table_levels=None):
     """vk: dict of wire images (alpha_g1, beta_g1, beta_g2, gamma_g2, delta_g1, delta_g2, ic[]);
-    h/l/a/b_g1: [n,104] uint8, b_g2: [n,200] uint8 — bellman `Parameters` vectors."""
+    h/l/a/b_g1: [n,104] uint8, b_g2: [n,200] uint8 — bellman `Parameters` vectors.
+    table_levels: fixed-base table levels of the key (1 = no tables, 0 = as many as fit in free device memory);
+    None = the BZK_TABLE_LEVELS environment value, else 0.  Proofs are the same for every level count."""
     hb, lb, ab, b1b = (ctx.g1_bases(np.ascontiguousarray(x, dtype=np.uint8).reshape(-1, G1_BYTES)) for x in (h, l, a, b_g1))
     b2b = ctx.g2_bases(np.ascontiguousarray(b_g2, dtype=np.uint8).reshape(-1, G2_BYTES))
-    return _make_pk(ctx, vk, hb, lb, ab, b1b, b2b)
+    return _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels)
 
 
-def _make_pk(ctx, vk, hb, lb, ab, b1b, b2b):
+def _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels=None):
     out = ct.c_void_p()
     pts = [np.ascontiguousarray(vk[k], dtype=np.uint8) for k in ("alpha_g1", "beta_g1", "beta_g2", "delta_g1", "delta_g2")]
     ctx._check(ctx._l.bzk_groth16_params_create(ctx._h, *[_host_ptr(p) for p in pts], hb._h, lb._h, ab._h, b1b._h, b2b._h, ct.byref(out)))
     for b in (hb, lb, ab, b1b, b2b):
         b._h = None  # adopted by the params handle
     pk = ProvingKey(ctx, out, vk)
-    import os
-    lv = os.environ.get("BZK_TABLE_LEVELS")   # development override: 1 = no tables
-    if lv is None or int(lv) != 1:
-        pk.precompute(int(lv) if lv else 0)
+    if table_levels is None:
+        import os
+        lv = os.environ.get("BZK_TABLE_LEVELS")   # development override: 1 = no tables
+        table_levels = int(lv) if lv else 0
+    if table_levels != 1:
+        pk.precompute(table_levels)
     return pk
 
 
@@ -401,21 +405,21 @@ def zkproof_blob(proof_bytes):
 # ------------------------------------------------------------------------------------------------
 # trusted setup on the GPU (bellman `generate_parameters`, explicit toxic waste)
 # ------------------------------------------------------------------------------------------------
-def setup_gpu(ctx: Context, r1cs: R1CS, toxic, g1_image, g2_image):
+def setup_gpu(ctx: Context, r1cs: R1CS, toxic, g1_image, g2_image, table_levels=None):
     """toxic = [tau, alpha, beta, gamma, delta] as [5,4] Montgomery; g1/g2: generator wire images.
     Returns (ProvingKey, vk dict).  All field/group work runs in libbzk kernels; numpy only moves
-    and reorders data."""
+    and reorders data.  table_levels: as in proving_key_from_host."""
     import torch
     # torch slicing / indexing kernels and libbzk kernels interleave below: put both on one stream
     ctx.use_torch_stream()
     try:
-        return _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image)
+        return _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels)
     finally:
         torch.cuda.synchronize()
         ctx.use_own_stream()
 
 
-def _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image):
+def _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels):
     import torch
     t = torch
     toxic = np.ascontiguousarray(toxic, dtype=np.uint64).reshape(5, 4)
@@ -513,7 +517,7 @@ def _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image):
     b2b = ctx.g2_bases_from_dev(b2_pts.contiguous() if len(b_idx) else t.empty((1, G2_BYTES), dtype=t.uint8, device="cuda"), len(b_idx))
     ctx.synchronize()
     host = {"h": h_pts, "l": l_pts, "a": a_pts, "b_g1": b1_pts, "b_g2": b2_pts}
-    pk = _make_pk(ctx, vk, hb, lb, ab, b1b, b2b)
+    pk = _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels)
     pk.device_images = host  # wire images kept for tests / export
     return pk, vk
 

@@ -73,6 +73,15 @@ uint64_t bzk_ctx_stage_ms(const bzk_ctx *ctx, float *last_ms, double *sum_ms, ui
  * group elements for any value; it is a speed knob (0..6; negative = the library default, currently 0 for both groups —
  * see DESIGN.md for the measurements). */
 int32_t bzk_ctx_set_msm_affine_rounds(bzk_ctx *ctx, int32_t g1_rounds, int32_t g2_rounds);
+/* Window c of the fixed-base tables that bzk_g*_bases_precompute / bzk_groth16_params_precompute build from now on on this
+ * context: 0 lets the planner choose (or the BZK_TABLE_C environment value, read once per process), 8..23 forces it;
+ * anything else is BZK_ERR_BAD_ARG.  Results are the same group elements for any window. */
+int32_t bzk_ctx_set_msm_table_window(bzk_ctx *ctx, uint32_t c);
+/* The plan of the last single MSM run on this context (bzk_msm_g*, bzk_msm_g*_resident[_dev]; not the Groth16 driver's
+ * concurrent sums): out = { c, W, T, G, NB, slice, nbits, long_len } — window bits, windows, table levels in use, bucket
+ * groups, buckets per group, buckets per reduction slice, bits of the slice index, and the number of bucket runs queued
+ * for the CTA-wide fold (read back only while bzk_ctx_set_timing is on, else 0).  W = 0: empty sum or no MSM yet. */
+int32_t bzk_ctx_last_msm_plan(const bzk_ctx *ctx, uint32_t out[8]);
 /* kernels launched through this ctx since creation (bench.py's `gpu_launches`) */
 uint64_t bzk_ctx_launch_count(const bzk_ctx *ctx);
 

@@ -65,6 +65,24 @@ def test_packed_transaction_structs_match_the_header(tmp_path):
         assert [dt.fields[f][1] for f in fs] == [int(o) for o in offs], name
 
 
+def test_plan_hooks_are_typed_and_refuse_bad_arguments():
+    """bzk_ctx_set_msm_table_window / bzk_ctx_last_msm_plan: typed as the header declares them, and a missing context or
+    output buffer is refused before anything is touched (the window range is checked on a real context in the gpu tier)."""
+    from bazuka_b200 import _lib
+    lib = _lib.load()
+    h = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "bzk.h")).read(), flags=re.S)
+    assert "int32_t bzk_ctx_set_msm_table_window(bzk_ctx *ctx, uint32_t c);" in h
+    assert "int32_t bzk_ctx_last_msm_plan(const bzk_ctx *ctx, uint32_t out[8]);" in h
+    assert _lib.SIGNATURES["bzk_ctx_set_msm_table_window"] == (ct.c_int32, [ct.c_void_p, ct.c_uint32])
+    assert _lib.SIGNATURES["bzk_ctx_last_msm_plan"] == (ct.c_int32, [ct.c_void_p, ct.c_void_p])
+    out = np.full(8, 7, dtype=np.uint32)
+    assert lib.bzk_ctx_last_msm_plan(None, out.ctypes.data_as(ct.c_void_p)) == -1
+    assert (out == 7).all()
+    for c in (0, 1, 7, 8, 23, 24, 0xFFFFFFFF):
+        assert lib.bzk_ctx_set_msm_table_window(None, c) == -1
+    assert lib.bzk_abi_version() == (1 << 16) | 1
+
+
 def test_no_cpu_fallback_without_gpu():
     import torch
     import bazuka_b200 as B

@@ -104,6 +104,43 @@ def test_prover_2_18_domain_vs_oracle(ctx, cref):
     assert (blob == GC.proof_bytes(*GC.prove(ni, na, mats, cpk, inputs, aux, r, s))).all()
 
 
+def test_proofs_do_not_depend_on_table_levels(ctx, cref):
+    """A key's fixed-base tables get as many levels as fit in the device memory free when it is built, so the same key
+    runs different MSM plans on different days.  One 2^16-domain circuit, one oracle proof on the key images, and the GPU
+    key built at every level count from 1 to 16: every proof is byte-equal to the oracle's, and the sweep ran at least
+    four distinct table plans (read from stand-alone copies of the key's columns tabled at the same level counts)."""
+    from bazuka_b200 import synth
+    from oracle import groth16_c as GC
+    ni, na, mats, inputs, aux = synth.build(64, 100, seed=23, ops=synth.GpuOps(ctx))
+    BG, pr = _prover(ctx, ni, na, mats)
+    assert pr.log_m == 16
+    tox = cref.fr_random(51, 5)
+    pk, vk = BG.setup_gpu(ctx, pr.r1cs, tox, cref.g1_generator(), cref.g2_generator(), table_levels=1)
+    cols = ("h", "l", "a", "b_g1", "b_g2")
+    imgs = {k: pk.device_images[k].cpu().numpy() for k in cols}
+    pk.free()
+    r, s = cref.fr_random(52, 2)
+    a_idx, b_idx = GC.density(ni, na, mats)
+    want = GC.proof_bytes(*GC.prove(ni, na, mats, dict(imgs, log_m=16, vk=vk, a_idx=a_idx, b_idx=b_idx), inputs, aux, r, s))
+    plans = set()
+    for levels in (1, 2, 3, 4, 5, 6, 8, 12, 16):
+        pk = BG.proving_key_from_host(ctx, vk, *(imgs[k] for k in cols), table_levels=levels)
+        blob, _ = pr.prove(pk, inputs, aux, r, s)
+        pk.free()
+        assert (blob == want).all(), levels
+        for k in cols:
+            rb = ctx.g2_bases(imgs[k]) if k == "b_g2" else ctx.g1_bases(imgs[k])
+            rb.precompute(levels)
+            sc = cref.fr_random(60, len(rb))
+            (ctx.msm_g2_resident if k == "b_g2" else ctx.msm_g1_resident)(rb, sc)
+            p = ctx.last_msm_plan()
+            if p["T"] > 1:
+                plans.add((p["c"], p["T"], p["G"]))
+            rb.free()
+    print(f"\ntable plans run by the key's columns over levels 1..16: {sorted(plans)}")
+    assert len(plans) >= 4, plans
+
+
 def test_base_sharded_partials_fold_to_the_same_proof(ctx, cref):
     """schedule (S) of SURVEY.md §8e on one GPU: the proving key cut into 3 contiguous base shards, each shard's
     four partial sums from `bzk_groth16_prove_partial`, folded with the host group law and finalised —
