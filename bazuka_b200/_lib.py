@@ -14,7 +14,8 @@ PARAMS_PATH = os.path.join(HERE, "data", "poseidon_params.bin")
 BZK_OK = 0
 ERRORS = {
     -1: "BZK_ERR_BAD_ARG", -2: "BZK_ERR_CUDA", -3: "BZK_ERR_OOM", -4: "BZK_ERR_NOT_ON_CURVE",
-    -5: "BZK_ERR_NO_PARAMS", -6: "BZK_ERR_NO_DEVICE", -7: "BZK_ERR_UNSAT",
+    -5: "BZK_ERR_NO_PARAMS", -6: "BZK_ERR_NO_DEVICE", -7: "BZK_ERR_UNSAT", -8: "BZK_ERR_BAD_ENCODING",
+    -9: "BZK_ERR_NOT_IN_SUBGROUP",
 }
 
 
@@ -84,6 +85,9 @@ SIGNATURES = {
     "bzk_groth16_prove_dev": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "bzk_groth16_stage_ms": (_i32, [_vp, _vp]),
     "bzk_groth16_params_precompute": (_i32, [_vp, _vp, ct.c_uint32, ct.c_uint32]),
+    "bzk_groth16_params_file_info": (_i32, [_vp, _sz, _vp]),
+    "bzk_groth16_params_read": (_i32, [_vp, _vp, _sz, _i32] + [_vp] * 7 + [_sz, ct.POINTER(_vp)]),
+    "bzk_groth16_params_write": (_i32, [_vp, _vp, _vp, _vp, _sz, _vp, _sz, ct.POINTER(_sz)]),
     "bzk_g1_bases_precompute": (_i32, [_vp, _vp, ct.c_uint32]),
     "bzk_g2_bases_precompute": (_i32, [_vp, _vp, ct.c_uint32]),
     "bzk_g1_bases_levels": (ct.c_uint32, [_vp]),

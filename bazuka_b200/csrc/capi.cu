@@ -102,6 +102,8 @@ const char *bzk_strerror(int32_t s) {
         case BZK_ERR_NO_PARAMS: return "Poseidon parameters not loaded";
         case BZK_ERR_NO_DEVICE: return "no CUDA device (libbzk has no CPU path)";
         case BZK_ERR_UNSAT: return "unsatisfied constraint system";
+        case BZK_ERR_BAD_ENCODING: return "bad key file encoding";
+        case BZK_ERR_NOT_IN_SUBGROUP: return "point not in the prime-order subgroup";
         default: return "unknown status";
     }
 }

@@ -95,6 +95,17 @@ struct bzk_g2_bases {
     uint32_t tab_c = 0, tab_T = 1, tab_G = 0;
 };
 
+// A proving key (groth16.cu; read from / written to bellman's file format by params_io.cu).
+struct bzk_groth16_params {
+    bzk::G1Affine alpha_g1, beta_g1, delta_g1;
+    bzk::G2Affine beta_g2, delta_g2;
+    bzk_g1_bases *h = nullptr, *l = nullptr, *a = nullptr, *b1 = nullptr;
+    bzk_g2_bases *b2 = nullptr;
+    // base sharding (SURVEY.md §8e): this handle holds the contiguous range
+    // [len*rank/world, len*(rank+1)/world) of each of the five base vectors
+    uint32_t rank = 0, world = 1;
+};
+
 namespace bzk {
 // what one MSM call sees of a base vector: the sub-range [off, off + n) of a (possibly multi-level) table
 template <class F>

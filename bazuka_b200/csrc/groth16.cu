@@ -46,16 +46,6 @@ struct bzk_r1cs {
     uint64_t a_len = 0, b_len = 0;
 };
 
-struct bzk_groth16_params {
-    bzk::G1Affine alpha_g1, beta_g1, delta_g1;
-    bzk::G2Affine beta_g2, delta_g2;
-    bzk_g1_bases *h = nullptr, *l = nullptr, *a = nullptr, *b1 = nullptr;
-    bzk_g2_bases *b2 = nullptr;
-    // base sharding (SURVEY.md §8e): this handle holds the contiguous range
-    // [len*rank/world, len*(rank+1)/world) of each of the five base vectors
-    uint32_t rank = 0, world = 1;
-};
-
 struct Groth16Partials {  // the four sums a proof is assembled from (wire images)
     bzk_g1_affine *a_sum, *b1_sum, *hl_sum;
     bzk_g2_affine *b2_sum;

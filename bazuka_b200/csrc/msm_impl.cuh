@@ -464,21 +464,14 @@ static __global__ void __launch_bounds__(256) k_pack_g1(const uint8_t *__restric
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     G1Affine p = load_g1_image(images + i * 104);
-    if (bad && !p.is_inf()) {
-        Fp rhs = p.x.sqr() * p.x + Fp::from_u32(4);
-        if (p.y.sqr() != rhs) atomicAdd(bad, 1u);
-    }
+    if (bad && !p.is_inf() && !on_curve(p)) atomicAdd(bad, 1u);
     store_vec(out + i, p);
 }
 static __global__ void __launch_bounds__(128) k_pack_g2(const uint8_t *__restrict__ images, size_t n, G2Affine *__restrict__ out, uint32_t *bad) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     G2Affine p = load_g2_image(images + i * 200);
-    if (bad && !p.is_inf()) {
-        Fp four = Fp::from_u32(4);
-        Fp2 rhs = p.x.sqr() * p.x + Fp2{four, four};
-        if (p.y.sqr() != rhs) atomicAdd(bad, 1u);
-    }
+    if (bad && !p.is_inf() && !on_curve(p)) atomicAdd(bad, 1u);
     store_vec(out + i, p);
 }
 
@@ -498,34 +491,6 @@ static __global__ void __launch_bounds__(256) k_random_fr(uint64_t seed, size_t 
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     store_vec(out + i, splitmix_fr_canonical(seed, i).to_mont());
-}
-
-// ---------------------------------------------------------------------------------------------
-// host: generator constants (canonical big-endian hex -> Montgomery)
-// ---------------------------------------------------------------------------------------------
-static Fp fp_from_hex(const char *hex96) {
-    Fp v;
-    for (int i = 0; i < 12; i++) {
-        uint32_t x = 0;
-        for (int k = 0; k < 8; k++) {
-            char ch = hex96[(11 - i) * 8 + k];
-            x = (x << 4) | (uint32_t)(ch <= '9' ? ch - '0' : (ch | 32) - 'a' + 10);
-        }
-        v.l[i] = x;
-    }
-    return v.to_mont();
-}
-static G1Affine g1_generator() {
-    return G1Affine{
-        fp_from_hex("17f1d3a73197d7942695638c4fa9ac0fc3688c4f9774b905a14e3a3f171bac586c55e83ff97a1aeffb3af00adb22c6bb"),
-        fp_from_hex("08b3f481e3aaa0f1a09e30ed741d8ae4fcf5e095d5d00af600db18cb2c04b3edd03cc744a2888ae40caa232946c5e7e1")};
-}
-static G2Affine g2_generator() {
-    return G2Affine{
-        Fp2{fp_from_hex("024aa2b2f08f0a91260805272dc51051c6e47ad4fa403b02b4510b647ae3d1770bac0326a805bbefd48056c8c121bdb8"),
-            fp_from_hex("13e02b6052719f607dacd3a088274f65596bd0d09920b61ab5da61bbdc7f5049334cf11213945d57e5ac7d055d042b7e")},
-        Fp2{fp_from_hex("0ce5d527727d6e118cc9cdc6da2e351aadfd9baa8cbdd3a76d429a695160d12c923ac9cc3baca289e193548608b82801"),
-            fp_from_hex("0606c4a02ea734cc32acd2b02bc28b99cb3e287e85a763af267492ab572e99ab3f370d275cec1da1aaa9075ff05f79be")}};
 }
 
 // wire image (host) <-> Affine<F>

@@ -8,6 +8,9 @@ production boundary: `MpnWork` in, `ZkProof::Groth16` out, /root/reference/src/m
   setup_gpu     bellman `generate_parameters` with explicit toxic waste, computed with libbzk kernels
                 (iNTT for the Lagrange basis, transposed SpMV, fixed-base multiplications); used to
                 make keys for synthetic circuits — production keys come from the ceremony
+  read_parameters / write_parameters
+                bellman's `Parameters::read` / `Parameters::write` file image <-> a resident ProvingKey, every point
+                decoded (and, checked, tested for the curve and the prime-order subgroup) on the GPU
   Prover.prove  -> 387-byte `Groth16Proof` bincode image (bit-exact vs the CPU prover for equal
                 (params, r, s, witness))
 """
@@ -126,7 +129,11 @@ def _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels=None):
     ctx._check(ctx._l.bzk_groth16_params_create(ctx._h, *[_host_ptr(p) for p in pts], hb._h, lb._h, ab._h, b1b._h, b2b._h, ct.byref(out)))
     for b in (hb, lb, ab, b1b, b2b):
         b._h = None  # adopted by the params handle
-    pk = ProvingKey(ctx, out, vk)
+    return _with_tables(ProvingKey(ctx, out, vk), table_levels)
+
+
+def _with_tables(pk, table_levels):
+    """the fixed-base table policy of proving_key_from_host"""
     if table_levels is None:
         import os
         lv = os.environ.get("BZK_TABLE_LEVELS")   # development override: 1 = no tables
@@ -134,6 +141,72 @@ def _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels=None):
     if table_levels != 1:
         pk.precompute(table_levels)
     return pk
+
+
+# ------------------------------------------------------------------------------------------------
+# bellman `Parameters` files (`Parameters::write` / `Parameters::read`, layout in csrc/params_io.cu)
+# ------------------------------------------------------------------------------------------------
+def _file_bytes(src):
+    """a path (memory-mapped, never loaded whole) or a bytes-like object -> uint8 array"""
+    import os
+    if isinstance(src, (str, os.PathLike)):
+        if os.path.getsize(src) == 0:
+            return np.zeros(0, dtype=np.uint8)
+        return np.memmap(src, dtype=np.uint8, mode="r")
+    if isinstance(src, np.ndarray):
+        return np.ascontiguousarray(src).reshape(-1).view(np.uint8)
+    return np.frombuffer(memoryview(src).cast("B"), dtype=np.uint8)
+
+
+PARAMS_FILE_INFO = np.dtype([(k, np.uint64) for k in ("n_ic", "n_h", "n_l", "n_a", "n_b_g1", "n_b_g2", "bytes")])
+
+
+def parameters_info(src):
+    """the header of a bellman `Parameters` file (bzk_groth16_params_file_info): point counts and the byte count they imply"""
+    from . import _lib
+    lib = _lib.load()
+    buf = _file_bytes(src)
+    out = np.zeros(1, dtype=PARAMS_FILE_INFO)
+    st = lib.bzk_groth16_params_file_info(_host_ptr(buf) if buf.size else None, buf.size, _host_ptr(out))
+    if st != 0:
+        raise _lib.BzkError(st, "groth16_params_file_info")
+    return {k: int(out[0][k]) for k in PARAMS_FILE_INFO.names}
+
+
+def read_parameters(ctx, src, checked=True, table_levels=None):
+    """bellman `Parameters::read(src, checked)` onto the GPU -> (ProvingKey, vk dict of wire images).  checked=True tests
+    every point for the curve equation and the prime-order subgroup (on the GPU); the verifying key is checked either way.
+    table_levels: as in proving_key_from_host.  A refused file raises BzkError naming the first bad point."""
+    buf = _file_bytes(src)
+    n_ic = parameters_info(buf)["n_ic"]
+    g1 = {k: np.zeros(G1_BYTES, np.uint8) for k in ("alpha_g1", "beta_g1", "delta_g1")}
+    g2 = {k: np.zeros(G2_BYTES, np.uint8) for k in ("beta_g2", "gamma_g2", "delta_g2")}
+    ic = np.zeros((max(n_ic, 1), G1_BYTES), np.uint8)
+    out = ct.c_void_p()
+    ctx._check(ctx._l.bzk_groth16_params_read(ctx._h, _host_ptr(buf), buf.size, int(bool(checked)), _host_ptr(g1["alpha_g1"]),
+                                              _host_ptr(g1["beta_g1"]), _host_ptr(g2["beta_g2"]), _host_ptr(g2["gamma_g2"]),
+                                              _host_ptr(g1["delta_g1"]), _host_ptr(g2["delta_g2"]), _host_ptr(ic), n_ic, ct.byref(out)))
+    vk = dict(g1, **g2, ic=ic[:n_ic])
+    return _with_tables(ProvingKey(ctx, out, vk), table_levels), vk
+
+
+def write_parameters(ctx, pk, dest=None):
+    """bellman `Parameters::write` of a key (level 0 of each vector, whatever its tables) -> a uint8 array, or into the file
+    `dest` (memory-mapped at its exact size), returning the path."""
+    ic = np.ascontiguousarray(pk.vk["ic"], dtype=np.uint8).reshape(-1, G1_BYTES)
+    gamma = np.ascontiguousarray(pk.vk["gamma_g2"], dtype=np.uint8)
+    n = ct.c_size_t()
+    args = (ctx._h, pk._h, _host_ptr(gamma), _host_ptr(ic), len(ic))
+    ctx._check(ctx._l.bzk_groth16_params_write(*args, None, 0, ct.byref(n)))
+    if dest is None:
+        out = np.empty(n.value, dtype=np.uint8)
+        ctx._check(ctx._l.bzk_groth16_params_write(*args, _host_ptr(out), out.size, ct.byref(n)))
+        return out
+    out = np.memmap(dest, dtype=np.uint8, mode="w+", shape=(n.value,))
+    ctx._check(ctx._l.bzk_groth16_params_write(*args, _host_ptr(out), out.size, ct.byref(n)))
+    out.flush()
+    del out
+    return dest
 
 
 class Prover:

@@ -46,6 +46,8 @@ typedef struct bzk_g2_bases bzk_g2_bases;
 #define BZK_ERR_NO_PARAMS (-5)     /* Poseidon parameter table not loaded */
 #define BZK_ERR_NO_DEVICE (-6)     /* no CUDA device: the library never falls back to the CPU */
 #define BZK_ERR_UNSAT (-7)         /* witness does not satisfy the constraint system */
+#define BZK_ERR_BAD_ENCODING (-8)  /* a key file image is truncated or holds a bad flag, a non-canonical coordinate or a point at infinity */
+#define BZK_ERR_NOT_IN_SUBGROUP (-9) /* a point is on the curve but not in the prime-order subgroup */
 
 const char *bzk_strerror(int32_t status);
 const char *bzk_last_error(const bzk_ctx *ctx);
@@ -235,6 +237,28 @@ int32_t bzk_groth16_prove_dev(bzk_ctx *ctx, const bzk_groth16_params *params, co
 /* Fixed-base tables for the five base vectors of a key; max_levels = 0: as many levels (<= 16) as fit in
  * mem_fraction_percent % (0 = 50) of the free device memory.  See bzk_g1_bases_precompute. */
 int32_t bzk_groth16_params_precompute(bzk_ctx *ctx, bzk_groth16_params *params, uint32_t max_levels, uint32_t mem_fraction_percent);
+
+/* Proving keys as bellman 0.14 keeps them on disk: the image `Parameters::write` makes and `Parameters::read` takes
+ * (layout in csrc/params_io.cu).  Points stream through two fixed staging chunks into the key's resident vectors, so
+ * device memory beyond the key is two chunks; every point is decoded and, when checked, tested on the GPU.
+ *   file_info  host only, no context: the lengths the image states and the byte count they imply (`bytes` may be less
+ *              than len: nothing after b_g2 is read); BZK_ERR_BAD_ENCODING when the image is shorter than that.
+ *   read       checked != 0: `Parameters::read(.., true)` (curve equation and prime-order subgroup for every point),
+ *              0: `read(.., false)`; the verifying key is checked either way.  The vk points come out as wire images
+ *              (ic[ic_cap], ic_cap >= n_ic) and the key as a handle like bzk_groth16_params_create makes (tables:
+ *              bzk_groth16_params_precompute afterwards).  On a refusal bzk_last_error names the first bad point in file
+ *              order ("l[65536]: not in the prime-order subgroup"): BZK_ERR_BAD_ENCODING (also |b_g1| != |b_g2|),
+ *              BZK_ERR_NOT_ON_CURVE or BZK_ERR_NOT_IN_SUBGROUP; nothing stays allocated.
+ *   write      the key's file image, level 0 of each vector whatever its table levels; out == NULL: *len = size only.
+ *              gamma_g2 and ic are not held by the handle.  A shard (set_shard, world > 1) is BZK_ERR_BAD_ARG. */
+typedef struct { uint64_t n_ic, n_h, n_l, n_a, n_b_g1, n_b_g2, bytes; } bzk_params_file_info;
+int32_t bzk_groth16_params_file_info(const uint8_t *bytes, size_t len, bzk_params_file_info *out);
+int32_t bzk_groth16_params_read(bzk_ctx *ctx, const uint8_t *bytes, size_t len, int32_t checked,
+                                bzk_g1_affine *alpha_g1, bzk_g1_affine *beta_g1, bzk_g2_affine *beta_g2, bzk_g2_affine *gamma_g2,
+                                bzk_g1_affine *delta_g1, bzk_g2_affine *delta_g2, bzk_g1_affine *ic, size_t ic_cap,
+                                bzk_groth16_params **out);
+int32_t bzk_groth16_params_write(bzk_ctx *ctx, const bzk_groth16_params *params, const bzk_g2_affine *gamma_g2,
+                                 const bzk_g1_affine *ic, size_t n_ic, uint8_t *out, size_t cap, size_t *len);
 
 /* Stage times of the last prove call made while bzk_ctx_set_timing was on (CUDA events): milliseconds after the start
  * of the call at which [1] z upload + the three SpMVs finished, [2] the quotient pipeline (7 NTTs), [3] the h sum (main
