@@ -274,6 +274,35 @@ __device__ __forceinline__ void store_g2_image(uint8_t *img, const G2Affine &p) 
     w[24] = 0;
 }
 
+// ---- wire <-> packed conversions (host): bzk_g1_affine / bzk_g2_affine <-> G1Affine / G2Affine --------------------------
+// The same images as above; the identity is written with y = Montgomery one and the flag set.
+inline G1Affine from_wire(const bzk_g1_affine *img) {
+    if (img->infinity) return G1Affine::inf();
+    G1Affine p;
+    memcpy(p.x.l, img->x, 48);
+    memcpy(p.y.l, img->y, 48);
+    return p;
+}
+inline G2Affine from_wire(const bzk_g2_affine *img) {
+    if (img->infinity) return G2Affine::inf();
+    G2Affine p;
+    memcpy(p.x.c0.l, img->x, 48); memcpy(p.x.c1.l, img->x + 6, 48);
+    memcpy(p.y.c0.l, img->y, 48); memcpy(p.y.c1.l, img->y + 6, 48);
+    return p;
+}
+inline void to_wire(bzk_g1_affine *img, const G1Affine &p) {
+    memset(img, 0, sizeof *img);
+    if (p.is_inf()) { const Fp one = Fp::one(); memcpy(img->y, one.l, 48); img->infinity = 1; return; }
+    memcpy(img->x, p.x.l, 48);
+    memcpy(img->y, p.y.l, 48);
+}
+inline void to_wire(bzk_g2_affine *img, const G2Affine &p) {
+    memset(img, 0, sizeof *img);
+    if (p.is_inf()) { const Fp one = Fp::one(); memcpy(img->y, one.l, 48); img->infinity = 1; return; }
+    memcpy(img->x, p.x.c0.l, 48); memcpy(img->x + 6, p.x.c1.l, 48);
+    memcpy(img->y, p.y.c0.l, 48); memcpy(img->y + 6, p.y.c1.l, 48);
+}
+
 // 128-bit vector load/store of a field element / packed point from 16-byte aligned memory
 template <class T>
 __device__ __forceinline__ T load_vec(const T *p) {

@@ -16,9 +16,7 @@
 // built once at upload; all vectors stay in HBM between stages.
 #include "common.cuh"
 #include <algorithm>
-#include <chrono>
 #include <future>
-#include <cstdlib>
 
 namespace bzk {
 int32_t precompute_g1(bzk_ctx *ctx, bzk_g1_bases *b, uint32_t max_levels);
@@ -44,20 +42,6 @@ struct bzk_r1cs {
     bzk::DevCsr m[3];
     uint32_t *d_a_idx = nullptr, *d_b_idx = nullptr;  // indices into z for the A / B sums
     uint64_t a_len = 0, b_len = 0;
-};
-
-struct Groth16Partials {  // the four sums a proof is assembled from (wire images)
-    bzk_g1_affine *a_sum, *b1_sum, *hl_sum;
-    bzk_g2_affine *b2_sum;
-};
-
-// sharded schedule with the quotient split over the ranks: the call is cut in two around the exchange of polynomials
-struct Groth16Split {
-    int phase;              // 1 = begin (z, this rank's share of the evaluation vectors on the coset, the four witness sums enqueued)
-                            // 2 = finish (h sum over this rank's slice of the quotient, folds)
-    uint32_t poly_mask;     // begin: bit s set = this rank transforms evaluation vector s (a, b, c)
-    bzk::Fr *evals[3];      // begin: caller's device buffers (domain size) for those vectors
-    const bzk::Fr *h_shard; // finish: the rank's slice [lo, hi) of the quotient's coefficients (device)
 };
 
 namespace bzk {
@@ -97,33 +81,6 @@ __global__ void __launch_bounds__(64) k_fixed_base_g2(G2Affine base, const Fr *_
     store_g2_image(out + i * 200, scalar_mul(base, k.l).to_affine());
 }
 
-static G1Affine g1_from_img(const bzk_g1_affine *img) {
-    if (img->infinity) return G1Affine::inf();
-    G1Affine p;
-    memcpy(p.x.l, img->x, 48);
-    memcpy(p.y.l, img->y, 48);
-    return p;
-}
-static G2Affine g2_from_img(const bzk_g2_affine *img) {
-    if (img->infinity) return G2Affine::inf();
-    G2Affine p;
-    memcpy(p.x.c0.l, img->x, 48); memcpy(p.x.c1.l, img->x + 6, 48);
-    memcpy(p.y.c0.l, img->y, 48); memcpy(p.y.c1.l, img->y + 6, 48);
-    return p;
-}
-static void g1_to_img(bzk_g1_affine *img, const G1Affine &p) {
-    memset(img, 0, sizeof *img);
-    if (p.is_inf()) { Fp one = Fp::one(); memcpy(img->y, one.l, 48); img->infinity = 1; return; }
-    memcpy(img->x, p.x.l, 48);
-    memcpy(img->y, p.y.l, 48);
-}
-static void g2_to_img(bzk_g2_affine *img, const G2Affine &p) {
-    memset(img, 0, sizeof *img);
-    if (p.is_inf()) { Fp one = Fp::one(); memcpy(img->y, one.l, 48); img->infinity = 1; return; }
-    memcpy(img->x, p.x.c0.l, 48); memcpy(img->x + 6, p.x.c1.l, 48);
-    memcpy(img->y, p.y.c0.l, 48); memcpy(img->y + 6, p.y.c1.l, 48);
-}
-
 static int32_t upload_csr(bzk_ctx *ctx, DevCsr &d, uint64_t nrows, const uint64_t *rp, const uint32_t *col, const bzk_fr *val) {
     d.nnz = rp[nrows];
     BZK_CUDA(ctx, cudaMalloc(&d.rowptr, (nrows + 1) * sizeof(uint64_t)));
@@ -139,6 +96,238 @@ static void free_r1cs(bzk_r1cs *r) {
     if (r->d_a_idx) cudaFree(r->d_a_idx);
     if (r->d_b_idx) cudaFree(r->d_b_idx);
     delete r;
+}
+
+// ---- the prover's stages; the C entry points below are compositions of them -------------------------------------------
+
+// the four sums a proof is assembled from (wire images)
+struct Groth16Partials {
+    bzk_g1_affine a, b1, hl;
+    bzk_g2_affine b2;
+};
+
+// this handle's slice [lo, lo + n) of the terms of each sum: all of them when world == 1, else the shard's
+struct Slices {
+    uint64_t h_lo, h_n, l_lo, l_n, a_lo, a_n, b_lo, b_n;
+};
+static int32_t shard_slices(const bzk_groth16_params *pk, const bzk_r1cs *cs, Slices *s) {
+    auto lo_of = [&](uint64_t len) { return len * pk->rank / pk->world; };
+    auto cnt_of = [&](uint64_t len) { return len * (pk->rank + 1) / pk->world - lo_of(len); };
+    const uint64_t h_len = ((uint64_t)1 << cs->log_m) - 1;
+    *s = {lo_of(h_len), cnt_of(h_len), lo_of(cs->num_aux), cnt_of(cs->num_aux), lo_of(cs->a_len), cnt_of(cs->a_len), lo_of(cs->b_len), cnt_of(cs->b_len)};
+    // a whole key's h may be longer than the domain needs; a shard's vectors are exactly its slices
+    if ((pk->world == 1 ? pk->h->n < s->h_n : pk->h->n != s->h_n) || pk->l->n != s->l_n || pk->a->n != s->a_n || pk->b1->n != s->b_n ||
+        pk->b2->n != s->b_n)
+        return BZK_ERR_BAD_ARG;
+    return BZK_OK;
+}
+
+// the staging arena: z | a, b, c evaluations (domain size) | the gathered A / B scalars | unsatisfied-row count
+struct Stage {
+    Fr *z, *ev[3], *gs_a, *gs_b;
+    uint32_t *bad;
+};
+static int32_t stage_arena(bzk_ctx *ctx, const bzk_r1cs *cs, Stage *sg) {
+    const uint64_t m = (uint64_t)1 << cs->log_m, gmax = std::max<uint64_t>(std::max(cs->a_len, cs->b_len), 1);
+    auto carve = [&](void *base) {
+        Carver cv(base);
+        sg->z = cv.take<Fr>(cs->num_inputs + cs->num_aux);
+        for (Fr *&e : sg->ev) e = cv.take<Fr>(m);
+        sg->gs_a = cv.take<Fr>(gmax);
+        sg->gs_b = cv.take<Fr>(gmax);
+        sg->bad = cv.take<uint32_t>(4);
+        return cv.used();
+    };
+    BZK_TRY(ensure_ws(ctx, &ctx->stage, &ctx->stage_bytes, carve(nullptr)));
+    carve(ctx->stage);
+    return BZK_OK;
+}
+
+// mark k of bzk_groth16_stage_ms, recorded on stream s when timing is on
+static void g16_mark(bzk_ctx *ctx, int k, cudaStream_t s) {
+    if (!ctx->timing) return;
+    if (!ctx->g16_ev[k]) cudaEventCreate(&ctx->g16_ev[k]);
+    cudaEventRecord(ctx->g16_ev[k], s);
+}
+
+// Starts a proof on the context (an open shard_begin is abandoned): z into the arena from `inputs` / `aux` (kind: host
+// images or already on the device), then the SpMVs into the evaluation vectors ev[s] that are not null.  Rows >= ncons
+// are the Input(i) * 0 = 0 rows appended to A, then zero padding.  With `check`, rows where a * b != c are refused.
+static int32_t witness_side(bzk_ctx *ctx, const bzk_r1cs *cs, const Stage &sg, const bzk_fr *inputs, const bzk_fr *aux, cudaMemcpyKind kind,
+                            Fr *const ev[3], bool check) {
+    cudaStream_t st = ctx->stream;
+    const uint64_t ni = cs->num_inputs, m = (uint64_t)1 << cs->log_m;
+    ctx->split_open = false;
+    ctx->g16_valid = false;
+    g16_mark(ctx, 0, st);
+    BZK_CUDA(ctx, cudaMemcpyAsync(sg.z, inputs, ni * sizeof(Fr), kind, st));
+    if (cs->num_aux) BZK_CUDA(ctx, cudaMemcpyAsync(sg.z + ni, aux, cs->num_aux * sizeof(Fr), kind, st));
+    for (int s = 0; s < 3; s++) {
+        if (!ev[s]) continue;
+        BZK_CUDA(ctx, cudaMemsetAsync(ev[s] + cs->ncons, 0, (m - cs->ncons) * sizeof(Fr), st));
+        if (cs->ncons) {
+            k_csr_spmv<<<div_up(cs->ncons, 256), 256, 0, st>>>(cs->m[s].rowptr, cs->m[s].col, cs->m[s].val, cs->ncons, sg.z, ev[s]);
+            BZK_LAUNCHED(ctx);
+        }
+    }
+    if (ev[0]) BZK_CUDA(ctx, cudaMemcpyAsync(ev[0] + cs->ncons, sg.z, ni * sizeof(Fr), cudaMemcpyDeviceToDevice, st));
+    if (!check || !cs->ncons) return BZK_OK;
+    BZK_CUDA(ctx, cudaMemsetAsync(sg.bad, 0, 4, st));
+    k_check_sat<<<div_up(cs->ncons, 256), 256, 0, st>>>(ev[0], ev[1], ev[2], cs->ncons, sg.bad);
+    BZK_LAUNCHED(ctx);
+    uint32_t bad = 0;
+    BZK_CUDA(ctx, cudaMemcpyAsync(&bad, sg.bad, 4, cudaMemcpyDeviceToHost, st));
+    BZK_CUDA(ctx, cudaStreamSynchronize(st));
+    if (bad) {
+        snprintf(ctx->err, sizeof ctx->err, "%u constraints unsatisfied by the witness", bad);
+        return BZK_ERR_UNSAT;
+    }
+    return BZK_OK;
+}
+
+// one sum's window sums on the host (sized for G2); the pinned block holds five, in the order h, l, a, b_g1, b_g2
+constexpr size_t kWinBytes = kMaxWinPoints * sizeof(G2Xyzz);
+
+// The five sums are independent once z is on the device (h additionally needs the quotient): the gathers and the l, a,
+// b_g1, b_g2 sums run on side streams with their own arenas, behind what the main stream has enqueued so far, while the
+// main stream goes on to the quotient and the h sum.  So the latency-bound phases of one MSM (bucket reduction, side-list
+// folding) overlap the throughput-bound phases of the others.
+static int32_t witness_sums(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const Stage &sg, const Slices &sl) {
+    for (int k = 0; k < 4; k++)
+        if (!ctx->aux_stream[k]) BZK_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->aux_stream[k], cudaStreamNonBlocking));
+    for (int k = 0; k < 3; k++)
+        if (!ctx->aux_ev[k]) BZK_CUDA(ctx, cudaEventCreateWithFlags(&ctx->aux_ev[k], cudaEventDisableTiming));
+    if (ctx->pinned_bytes < 5 * kWinBytes) {
+        if (ctx->pinned) cudaFreeHost(ctx->pinned);
+        ctx->pinned = nullptr;
+        BZK_CUDA(ctx, cudaHostAlloc(&ctx->pinned, 5 * kWinBytes, cudaHostAllocDefault));
+        ctx->pinned_bytes = 5 * kWinBytes;
+    }
+    char *hw = (char *)ctx->pinned;
+    MsmPlan *plan = ctx->g16_plan;
+    const uint64_t ni = cs->num_inputs;
+    cudaStream_t st = ctx->stream, s_l = ctx->aux_stream[0], s_a = ctx->aux_stream[1], s_b1 = ctx->aux_stream[2], s_b2 = ctx->aux_stream[3];
+    g16_mark(ctx, 1, st);
+    BZK_CUDA(ctx, cudaEventRecord(ctx->aux_ev[0], st));  // z and the evaluations are enqueued behind this point
+    BZK_CUDA(ctx, cudaStreamWaitEvent(s_l, ctx->aux_ev[0], 0));
+    BZK_CUDA(ctx, cudaStreamWaitEvent(s_a, ctx->aux_ev[0], 0));
+    BZK_CUDA(ctx, cudaStreamWaitEvent(s_b1, ctx->aux_ev[0], 0));
+    BZK_TRY(msm_g1_enqueue(ctx, s_l, &ctx->aux_ws[0], &ctx->aux_ws_bytes[0], bases_ref(pk->l), sg.z + ni + sl.l_lo, sl.l_n, hw + 1 * kWinBytes, &plan[1]));
+    k_gather_fr<<<div_up(cs->a_len, 256), 256, 0, s_a>>>(sg.z, cs->d_a_idx, cs->a_len, sg.gs_a);
+    BZK_LAUNCHED(ctx);
+    BZK_TRY(msm_g1_enqueue(ctx, s_a, &ctx->aux_ws[1], &ctx->aux_ws_bytes[1], bases_ref(pk->a), sg.gs_a + sl.a_lo, sl.a_n, hw + 2 * kWinBytes, &plan[2]));
+    if (cs->b_len) {
+        k_gather_fr<<<div_up(cs->b_len, 256), 256, 0, s_b1>>>(sg.z, cs->d_b_idx, cs->b_len, sg.gs_b);
+        BZK_LAUNCHED(ctx);
+    }
+    BZK_CUDA(ctx, cudaEventRecord(ctx->aux_ev[1], s_b1));
+    BZK_CUDA(ctx, cudaStreamWaitEvent(s_b2, ctx->aux_ev[1], 0));
+    BZK_TRY(msm_g1_enqueue(ctx, s_b1, &ctx->aux_ws[2], &ctx->aux_ws_bytes[2], bases_ref(pk->b1), sg.gs_b + sl.b_lo, sl.b_n, hw + 3 * kWinBytes, &plan[3]));
+    BZK_TRY(msm_g2_enqueue(ctx, s_b2, &ctx->aux_ws[3], &ctx->aux_ws_bytes[3], bases_ref(pk->b2), sg.gs_b + sl.b_lo, sl.b_n, hw + 4 * kWinBytes, &plan[4]));
+    for (int k = 0; k < 4; k++) g16_mark(ctx, 4 + k, ctx->aux_stream[k]);
+    return BZK_OK;
+}
+
+// the h sum over n quotient coefficients at src, on the main stream
+static int32_t h_sum(bzk_ctx *ctx, const bzk_groth16_params *pk, const Fr *src, uint64_t n) {
+    BZK_TRY(msm_g1_enqueue(ctx, ctx->stream, &ctx->ws, &ctx->ws_bytes, bases_ref(pk->h), src, n, ctx->pinned, &ctx->g16_plan[0]));
+    g16_mark(ctx, 3, ctx->stream);
+    return BZK_OK;
+}
+
+// Waits for the main stream and the four side streams, then folds the five window sets into the four sums.  The folds
+// are independent sub-millisecond jobs: they run on host threads instead of back to back.
+static int32_t collect(bzk_ctx *ctx, bzk_g1_affine *a_sum, bzk_g1_affine *b1_sum, bzk_g2_affine *b2_sum, bzk_g1_affine *hl_sum) {
+    BZK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (int k = 0; k < 4; k++) BZK_CUDA(ctx, cudaStreamSynchronize(ctx->aux_stream[k]));
+    if (ctx->timing) {
+        for (int k = 1; k < 8; k++) cudaEventElapsedTime(&ctx->g16_ms[k], ctx->g16_ev[0], ctx->g16_ev[k]);
+        ctx->g16_ms[0] = 0;
+        ctx->g16_valid = true;
+    }
+    const MsmPlan *plan = ctx->g16_plan;
+    const char *hw = (const char *)ctx->pinned;
+    bzk_g1_affine h, l;
+    auto f_b2 = std::async(std::launch::async, [&] { msm_g2_finish(&plan[4], hw + 4 * kWinBytes, b2_sum); });
+    auto f_a = std::async(std::launch::async, [&] { msm_g1_finish(&plan[2], hw + 2 * kWinBytes, a_sum); });
+    auto f_b1 = std::async(std::launch::async, [&] { msm_g1_finish(&plan[3], hw + 3 * kWinBytes, b1_sum); });
+    auto f_l = std::async(std::launch::async, [&] { msm_g1_finish(&plan[1], hw + 1 * kWinBytes, &l); });
+    msm_g1_finish(&plan[0], hw, &h);
+    f_l.get();
+    G1Xyzz hl = G1Xyzz::from_affine(from_wire(&h));
+    hl.madd(from_wire(&l));
+    to_wire(hl_sum, hl.to_affine());
+    f_b2.get(); f_a.get(); f_b1.get();
+    return BZK_OK;
+}
+
+// everything a proof enqueues for one witness: z and the three evaluations (checked if asked), the four witness sums on
+// the side streams, the quotient and the h sum on the main stream
+static int32_t enqueue_proof(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const bzk_fr *inputs, const bzk_fr *aux,
+                             cudaMemcpyKind kind, bool check) {
+    Slices sl;
+    Stage sg;
+    BZK_TRY(shard_slices(pk, cs, &sl));
+    BZK_TRY(stage_arena(ctx, cs, &sg));
+    BZK_TRY(witness_side(ctx, cs, sg, inputs, aux, kind, sg.ev, check));
+    BZK_TRY(witness_sums(ctx, pk, cs, sg, sl));
+    BZK_TRY(groth16_h_launch(ctx, sg.ev[0], sg.ev[1], sg.ev[2], cs->log_m));  // a <- the quotient's coefficients
+    g16_mark(ctx, 2, ctx->stream);
+    return h_sum(ctx, pk, sg.ev[0] + sl.h_lo, sl.h_n);
+}
+
+// bellman `create_proof`'s last lines, from the key's points, (r, s) and the four sums:
+//   A = r delta1 + alpha1 + a;  B = s delta2 + beta2 + b2;  C = rs delta1 + s alpha1 + r beta1 + s a + r b1 + (h + l)
+// `sums` fills in the four sums (it may wait for the GPU, or fail); the terms without them are computed meanwhile.
+template <class SumsFn>
+static int32_t proof_tail(const G1Affine &alpha1, const G1Affine &beta1, const G2Affine &beta2, const G1Affine &delta1, const G2Affine &delta2,
+                          const bzk_fr *r_mont, const bzk_fr *s_mont, SumsFn sums, bzk_g1_affine *proof_a, bzk_g2_affine *proof_b,
+                          bzk_g1_affine *proof_c) {
+    Fr r, s;
+    memcpy(r.l, r_mont, 32);
+    memcpy(s.l, s_mont, 32);
+    const Fr rs = (r * s).from_mont(), rc = r.from_mont(), sc = s.from_mont();
+    auto f_b = std::async(std::launch::async, [&] {
+        G2Xyzz t = scalar_mul(delta2, sc.l);
+        t.madd(beta2);
+        return t;
+    });
+    auto f_c = std::async(std::launch::async, [&] {
+        G1Xyzz t = scalar_mul(delta1, rs.l);
+        t.add(scalar_mul(alpha1, sc.l));
+        t.add(scalar_mul(beta1, rc.l));
+        return t;
+    });
+    G1Xyzz ga = scalar_mul(delta1, rc.l);
+    ga.madd(alpha1);
+    Groth16Partials p;
+    BZK_TRY(sums(&p));
+    const G1Affine a = from_wire(&p.a);
+    auto f_sa = std::async(std::launch::async, [&] { return scalar_mul(a, sc.l); });
+    const G1Xyzz rb1 = scalar_mul(from_wire(&p.b1), rc.l);
+    ga.madd(a);
+    G1Xyzz gc = f_c.get();
+    gc.add(f_sa.get());
+    gc.add(rb1);
+    gc.madd(from_wire(&p.hl));
+    G2Xyzz gb = f_b.get();
+    gb.madd(from_wire(&p.b2));
+    to_wire(proof_a, ga.to_affine());
+    to_wire(proof_b, gb.to_affine());
+    to_wire(proof_c, gc.to_affine());
+    return BZK_OK;
+}
+
+// a whole proof; kind: where `inputs` / `aux` live (host images, or already resident, e.g. written by bzk_witness_run_dev)
+static int32_t whole_proof(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const bzk_fr *inputs, const bzk_fr *aux,
+                           cudaMemcpyKind kind, const bzk_fr *r_mont, const bzk_fr *s_mont, int32_t check_satisfied, bzk_g1_affine *proof_a,
+                           bzk_g2_affine *proof_b, bzk_g1_affine *proof_c) {
+    if (!ctx || !pk || !cs || !inputs || (cs->num_aux && !aux) || !r_mont || !s_mont || !proof_a || !proof_b || !proof_c) return BZK_ERR_BAD_ARG;
+    if (pk->world != 1) return BZK_ERR_BAD_ARG;  // a shard can only produce partial sums
+    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+    BZK_TRY(enqueue_proof(ctx, pk, cs, inputs, aux, kind, check_satisfied != 0));
+    return proof_tail(pk->alpha_g1, pk->beta_g1, pk->beta_g2, pk->delta_g1, pk->delta_g2, r_mont, s_mont,
+                      [&](Groth16Partials *p) { return collect(ctx, &p->a, &p->b1, &p->b2, &p->hl); }, proof_a, proof_b, proof_c);
 }
 
 }  // namespace bzk
@@ -229,7 +418,7 @@ int32_t bzk_g1_fixed_base_mul_dev(bzk_ctx *ctx, const bzk_g1_affine *base, const
     if (!ctx || !base || (n && (!d_scalars || !d_out))) return BZK_ERR_BAD_ARG;
     BZK_CUDA(ctx, cudaSetDevice(ctx->device));
     if (n == 0) return BZK_OK;
-    k_fixed_base_g1<<<div_up(n, 128), 128, 0, ctx->stream>>>(g1_from_img(base), (const Fr *)d_scalars, n, (uint8_t *)d_out);
+    k_fixed_base_g1<<<div_up(n, 128), 128, 0, ctx->stream>>>(from_wire(base), (const Fr *)d_scalars, n, (uint8_t *)d_out);
     BZK_LAUNCHED(ctx);
     return BZK_OK;
 }
@@ -237,7 +426,7 @@ int32_t bzk_g2_fixed_base_mul_dev(bzk_ctx *ctx, const bzk_g2_affine *base, const
     if (!ctx || !base || (n && (!d_scalars || !d_out))) return BZK_ERR_BAD_ARG;
     BZK_CUDA(ctx, cudaSetDevice(ctx->device));
     if (n == 0) return BZK_OK;
-    k_fixed_base_g2<<<div_up(n, 64), 64, 0, ctx->stream>>>(g2_from_img(base), (const Fr *)d_scalars, n, (uint8_t *)d_out);
+    k_fixed_base_g2<<<div_up(n, 64), 64, 0, ctx->stream>>>(from_wire(base), (const Fr *)d_scalars, n, (uint8_t *)d_out);
     BZK_LAUNCHED(ctx);
     return BZK_OK;
 }
@@ -250,8 +439,8 @@ int32_t bzk_groth16_params_create(bzk_ctx *ctx, const bzk_g1_affine *alpha_g1, c
     if (b_g1->n != b_g2->n) return BZK_ERR_BAD_ARG;
     bzk_groth16_params *p = new (std::nothrow) bzk_groth16_params();
     if (!p) return BZK_ERR_OOM;
-    p->alpha_g1 = g1_from_img(alpha_g1); p->beta_g1 = g1_from_img(beta_g1); p->delta_g1 = g1_from_img(delta_g1);
-    p->beta_g2 = g2_from_img(beta_g2); p->delta_g2 = g2_from_img(delta_g2);
+    p->alpha_g1 = from_wire(alpha_g1); p->beta_g1 = from_wire(beta_g1); p->delta_g1 = from_wire(delta_g1);
+    p->beta_g2 = from_wire(beta_g2); p->delta_g2 = from_wire(delta_g2);
     p->h = h; p->l = l; p->a = a; p->b1 = b_g1; p->b2 = b_g2;
     *out = p;
     return BZK_OK;
@@ -266,230 +455,17 @@ int32_t bzk_groth16_params_free(bzk_ctx *ctx, bzk_groth16_params *p) {
     return BZK_OK;
 }
 
-// witness_kind: where `inputs` / `aux` live (cudaMemcpyHostToDevice: host images; cudaMemcpyDeviceToDevice:
-// already resident, e.g. written by bzk_witness_run_dev)
-static int32_t groth16_prove_impl(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const bzk_fr *inputs, const bzk_fr *aux,
-                                  cudaMemcpyKind witness_kind, const bzk_fr *r_mont, const bzk_fr *s_mont, int32_t check_satisfied,
-                                  bzk_g1_affine *proof_a, bzk_g2_affine *proof_b, bzk_g1_affine *proof_c,
-                                  const Groth16Partials *partial = nullptr, const Groth16Split *split = nullptr) {
-    const int phase = split ? split->phase : 0;
-    if (!ctx || !pk || !cs || (phase != 2 && (!inputs || (cs->num_aux && !aux)))) return BZK_ERR_BAD_ARG;
-    if (!partial && phase != 1 && (!r_mont || !s_mont || !proof_a || !proof_b || !proof_c)) return BZK_ERR_BAD_ARG;
-    if (!partial && phase != 1 && pk->world != 1) return BZK_ERR_BAD_ARG;  // a shard can only produce partial sums
-    if (phase == 2 && (!partial || !ctx->split_open || (!split->h_shard && pk->h->n))) return BZK_ERR_BAD_ARG;
-    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
-    // BZK_TRACE=1: host-side wall clock of the driver's phases on stderr (development aid)
-    static const bool trace = std::getenv("BZK_TRACE") != nullptr;
-    auto t_start = std::chrono::steady_clock::now();
-    auto lap = [&](const char *what) {
-        if (!trace) return;
-        auto now = std::chrono::steady_clock::now();
-        fprintf(stderr, "[bzk prove] %-28s %8.3f ms\n", what, std::chrono::duration<double, std::milli>(now - t_start).count());
-    };
-    const uint64_t ni = cs->num_inputs, na = cs->num_aux, nv = ni + na, m = (uint64_t)1 << cs->log_m;
-    // this handle's slice of each sum (the whole range when world == 1)
-    auto lo_of = [&](uint64_t len) { return len * pk->rank / pk->world; };
-    auto cnt_of = [&](uint64_t len) { return len * (pk->rank + 1) / pk->world - len * pk->rank / pk->world; };
-    const uint64_t h_lo = lo_of(m - 1), h_n = cnt_of(m - 1), l_lo = lo_of(na), l_n = cnt_of(na), a_lo = lo_of(cs->a_len), a_n = cnt_of(cs->a_len),
-                   b_lo = lo_of(cs->b_len), b_n = cnt_of(cs->b_len);
-    if ((pk->world == 1 ? pk->h->n < h_n : pk->h->n != h_n) || pk->l->n != l_n || pk->a->n != a_n || pk->b1->n != b_n || pk->b2->n != b_n)
-        return BZK_ERR_BAD_ARG;
-    // staging arena: z | a_ev | b_ev | c_ev | gathered scalars
-    const size_t gmax = std::max<uint64_t>(std::max(cs->a_len, cs->b_len), 1);
-    size_t need = 0;
-    {
-        Carver cv(nullptr);
-        cv.take<Fr>(nv); cv.take<Fr>(m); cv.take<Fr>(m); cv.take<Fr>(m); cv.take<Fr>(gmax); cv.take<Fr>(gmax); cv.take<uint32_t>(4);
-        need = cv.used();
-    }
-    BZK_TRY(ensure_ws(ctx, &ctx->stage, &ctx->stage_bytes, need));
-    Carver cv(ctx->stage);
-    Fr *z = cv.take<Fr>(nv), *ea = cv.take<Fr>(m), *eb = cv.take<Fr>(m), *ec = cv.take<Fr>(m), *gs_a = cv.take<Fr>(gmax), *gs_b = cv.take<Fr>(gmax);
-    uint32_t *d_bad = cv.take<uint32_t>(4);
-    cudaStream_t st = ctx->stream;
-    const bool timed = ctx->timing;
-    auto g16_mark = [&](int k, cudaStream_t s) {
-        if (!timed) return;
-        if (!ctx->g16_ev[k]) cudaEventCreate(&ctx->g16_ev[k]);
-        cudaEventRecord(ctx->g16_ev[k], s);
-    };
-    MsmPlan *plan = ctx->g16_plan;
-    constexpr size_t kWinBytes = kMaxWinPoints * sizeof(G2Xyzz);
-    if (phase != 2) {
-    ctx->split_open = false;
-    ctx->g16_valid = false;
-    g16_mark(0, st);
-    BZK_CUDA(ctx, cudaMemcpyAsync(z, inputs, ni * sizeof(Fr), witness_kind, st));
-    if (na) BZK_CUDA(ctx, cudaMemcpyAsync(z + ni, aux, na * sizeof(Fr), witness_kind, st));
-    // evaluations (rows >= ncons: the Input(i)*0=0 rows, then zero padding)
-    Fr *ev[3] = {ea, eb, ec};
-    if (phase == 1) {
-        for (int s = 0; s < 3; s++) {
-            if (((split->poly_mask >> s) & 1) && !split->evals[s]) return BZK_ERR_BAD_ARG;
-            ev[s] = ((split->poly_mask >> s) & 1) ? split->evals[s] : nullptr;
-        }
-        ea = ev[0];
-    }
-    for (int s = 0; s < 3; s++) {
-        if (!ev[s]) continue;
-        BZK_CUDA(ctx, cudaMemsetAsync(ev[s] + cs->ncons, 0, (m - cs->ncons) * sizeof(Fr), st));
-        if (cs->ncons) {
-            k_csr_spmv<<<div_up(cs->ncons, 256), 256, 0, st>>>(cs->m[s].rowptr, cs->m[s].col, cs->m[s].val, cs->ncons, z, ev[s]);
-            BZK_LAUNCHED(ctx);
-        }
-    }
-    if (ea) BZK_CUDA(ctx, cudaMemcpyAsync(ea + cs->ncons, z, ni * sizeof(Fr), cudaMemcpyDeviceToDevice, st));
-    if (check_satisfied && cs->ncons && phase == 0) {
-        BZK_CUDA(ctx, cudaMemsetAsync(d_bad, 0, 4, st));
-        k_check_sat<<<div_up(cs->ncons, 256), 256, 0, st>>>(ea, eb, ec, cs->ncons, d_bad);
-        BZK_LAUNCHED(ctx);
-        uint32_t bad = 0;
-        BZK_CUDA(ctx, cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
-        BZK_CUDA(ctx, cudaStreamSynchronize(st));
-        if (bad) {
-            snprintf(ctx->err, sizeof ctx->err, "%u constraints unsatisfied by the witness", bad);
-            return BZK_ERR_UNSAT;
-        }
-    }
-    // The five sums are independent once z is on the device (h additionally needs the quotient):
-    // l, a, b_g1, b_g2 run on side streams with their own arenas while the main stream does the
-    // NTT pipeline and the h sum, so the latency-bound phases of one MSM (bucket reduction, side-list
-    // folding) overlap the throughput-bound phases of the others.
-    for (int k = 0; k < 4; k++)
-        if (!ctx->aux_stream[k]) BZK_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->aux_stream[k], cudaStreamNonBlocking));
-    for (int k = 0; k < 3; k++)
-        if (!ctx->aux_ev[k]) BZK_CUDA(ctx, cudaEventCreateWithFlags(&ctx->aux_ev[k], cudaEventDisableTiming));
-    if (ctx->pinned_bytes < 5 * kWinBytes) {
-        if (ctx->pinned) cudaFreeHost(ctx->pinned);
-        ctx->pinned = nullptr;
-        BZK_CUDA(ctx, cudaHostAlloc(&ctx->pinned, 5 * kWinBytes, cudaHostAllocDefault));
-        ctx->pinned_bytes = 5 * kWinBytes;
-    }
-    char *hw = (char *)ctx->pinned;
-    lap("z + evaluations enqueued");
-    cudaStream_t s_l = ctx->aux_stream[0], s_a = ctx->aux_stream[1], s_b1 = ctx->aux_stream[2], s_b2 = ctx->aux_stream[3];
-    g16_mark(1, st);
-    BZK_CUDA(ctx, cudaEventRecord(ctx->aux_ev[0], st));  // z and the evaluations are enqueued behind this point
-    BZK_CUDA(ctx, cudaStreamWaitEvent(s_l, ctx->aux_ev[0], 0));
-    BZK_CUDA(ctx, cudaStreamWaitEvent(s_a, ctx->aux_ev[0], 0));
-    BZK_CUDA(ctx, cudaStreamWaitEvent(s_b1, ctx->aux_ev[0], 0));
-    BZK_TRY(msm_g1_enqueue(ctx, s_l, &ctx->aux_ws[0], &ctx->aux_ws_bytes[0], bases_ref(pk->l), z + ni + l_lo, l_n, hw + 1 * kWinBytes, &plan[1]));
-    k_gather_fr<<<div_up(cs->a_len, 256), 256, 0, s_a>>>(z, cs->d_a_idx, cs->a_len, gs_a);
-    BZK_LAUNCHED(ctx);
-    BZK_TRY(msm_g1_enqueue(ctx, s_a, &ctx->aux_ws[1], &ctx->aux_ws_bytes[1], bases_ref(pk->a), gs_a + a_lo, a_n, hw + 2 * kWinBytes, &plan[2]));
-    if (cs->b_len) {
-        k_gather_fr<<<div_up(cs->b_len, 256), 256, 0, s_b1>>>(z, cs->d_b_idx, cs->b_len, gs_b);
-        BZK_LAUNCHED(ctx);
-    }
-    BZK_CUDA(ctx, cudaEventRecord(ctx->aux_ev[1], s_b1));
-    BZK_CUDA(ctx, cudaStreamWaitEvent(s_b2, ctx->aux_ev[1], 0));
-    BZK_TRY(msm_g1_enqueue(ctx, s_b1, &ctx->aux_ws[2], &ctx->aux_ws_bytes[2], bases_ref(pk->b1), gs_b + b_lo, b_n, hw + 3 * kWinBytes, &plan[3]));
-    BZK_TRY(msm_g2_enqueue(ctx, s_b2, &ctx->aux_ws[3], &ctx->aux_ws_bytes[3], bases_ref(pk->b2), gs_b + b_lo, b_n, hw + 4 * kWinBytes, &plan[4]));
-    if (phase == 1) {
-        // this rank's evaluation vectors to the coset (ifft, then coset_fft); the pointwise step and the last transform
-        // happen on the rank that collects the three (bzk_groth16_h_combine_dev)
-        for (int s = 0; s < 3; s++)
-            if (ev[s]) BZK_TRY(groth16_to_coset_launch(ctx, ev[s], cs->log_m));
-        g16_mark(2, st);
-        BZK_CUDA(ctx, cudaStreamSynchronize(st));  // the caller hands the vectors to its transport next
-        ctx->split_open = true;
-        return BZK_OK;
-    }
-    BZK_TRY(groth16_h_launch(ctx, ea, eb, ec, cs->log_m));  // ea <- h coefficients
-    g16_mark(2, st);
-    }  // phase != 2
-    char *hw = (char *)ctx->pinned;
-    const Fr *h_src = phase == 2 ? split->h_shard : ea + h_lo;
-    ctx->split_open = false;
-    BZK_TRY(msm_g1_enqueue(ctx, st, &ctx->ws, &ctx->ws_bytes, bases_ref(pk->h), h_src, h_n, hw, &plan[0]));
-    g16_mark(3, st);
-    for (int k = 0; k < 4; k++) g16_mark(4 + k, ctx->aux_stream[k]);
-    lap("all kernels enqueued");
-    BZK_CUDA(ctx, cudaStreamSynchronize(st));
-    lap("main stream done");
-    for (int k = 0; k < 4; k++) BZK_CUDA(ctx, cudaStreamSynchronize(ctx->aux_stream[k]));
-    lap("side streams done");
-    if (timed) {
-        for (int k = 1; k < 8; k++) cudaEventElapsedTime(&ctx->g16_ms[k], ctx->g16_ev[0], ctx->g16_ev[k]);
-        ctx->g16_ms[0] = 0;
-        ctx->g16_valid = true;
-    }
-    // host tail: the five Horner folds and the (r, s) scalar multiplications are independent
-    // sub-millisecond jobs — run them on host threads instead of back to back
-    bzk_g1_affine h_ans, l_ans, a_ans, b1_ans;
-    bzk_g2_affine b2_ans;
-    if (partial) {  // sharded schedule: hand back this rank's four partial sums; the caller folds and finalises
-        auto p_b2 = std::async(std::launch::async, [&] { msm_g2_finish(&plan[4], hw + 4 * kWinBytes, partial->b2_sum); });
-        auto p_a = std::async(std::launch::async, [&] { msm_g1_finish(&plan[2], hw + 2 * kWinBytes, partial->a_sum); });
-        auto p_b1 = std::async(std::launch::async, [&] { msm_g1_finish(&plan[3], hw + 3 * kWinBytes, partial->b1_sum); });
-        auto p_l = std::async(std::launch::async, [&] { msm_g1_finish(&plan[1], hw + 1 * kWinBytes, &l_ans); });
-        msm_g1_finish(&plan[0], hw, &h_ans);
-        p_l.get();
-        G1Xyzz t = G1Xyzz::from_affine(g1_from_img(&h_ans));
-        t.madd(g1_from_img(&l_ans));
-        g1_to_img(partial->hl_sum, t.to_affine());
-        p_b2.get(); p_a.get(); p_b1.get();
-        lap("partial sums folded");
-        return BZK_OK;
-    }
-    Fr r, s;
-    memcpy(r.l, r_mont, 32);
-    memcpy(s.l, s_mont, 32);
-    const Fr rs = (r * s).from_mont(), rc = r.from_mont(), sc = s.from_mont();
-    auto f_b2 = std::async(std::launch::async, [&] {
-        msm_g2_finish(&plan[4], hw + 4 * kWinBytes, &b2_ans);
-        G2Xyzz gb = scalar_mul(pk->delta_g2, sc.l);
-        gb.madd(pk->beta_g2);
-        gb.madd(g2_from_img(&b2_ans));
-        return gb.to_affine();
-    });
-    auto f_a = std::async(std::launch::async, [&] {
-        msm_g1_finish(&plan[2], hw + 2 * kWinBytes, &a_ans);
-        return scalar_mul(g1_from_img(&a_ans), sc.l);  // s * a_sum
-    });
-    auto f_b1 = std::async(std::launch::async, [&] {
-        msm_g1_finish(&plan[3], hw + 3 * kWinBytes, &b1_ans);
-        return scalar_mul(g1_from_img(&b1_ans), rc.l);  // r * b1_sum
-    });
-    auto f_hl = std::async(std::launch::async, [&] {
-        msm_g1_finish(&plan[0], hw, &h_ans);
-        msm_g1_finish(&plan[1], hw + 1 * kWinBytes, &l_ans);
-        G1Xyzz t = G1Xyzz::from_affine(g1_from_img(&h_ans));
-        t.madd(g1_from_img(&l_ans));
-        return t;  // h_sum + l_sum
-    });
-    auto f_c0 = std::async(std::launch::async, [&] {
-        G1Xyzz t = scalar_mul(pk->delta_g1, rs.l);
-        t.add(scalar_mul(pk->alpha_g1, sc.l));
-        t.add(scalar_mul(pk->beta_g1, rc.l));
-        return t;  // r s delta + s alpha + r beta
-    });
-    G1Xyzz ga = scalar_mul(pk->delta_g1, rc.l);
-    ga.madd(pk->alpha_g1);
-    G1Xyzz gc = f_c0.get();
-    gc.add(f_a.get());
-    gc.add(f_b1.get());
-    gc.add(f_hl.get());
-    ga.madd(g1_from_img(&a_ans));
-    const G2Affine gb_aff = f_b2.get();
-    lap("host folds + blinding tail");
-    g1_to_img(proof_a, ga.to_affine());
-    g2_to_img(proof_b, gb_aff);
-    g1_to_img(proof_c, gc.to_affine());
-    return BZK_OK;
-}
-
 int32_t bzk_groth16_prove(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const bzk_fr *inputs, const bzk_fr *aux,
                           const bzk_fr *r_mont, const bzk_fr *s_mont, int32_t check_satisfied,
                           bzk_g1_affine *proof_a, bzk_g2_affine *proof_b, bzk_g1_affine *proof_c) {
-    return groth16_prove_impl(ctx, pk, cs, inputs, aux, cudaMemcpyHostToDevice, r_mont, s_mont, check_satisfied, proof_a, proof_b, proof_c);
+    return whole_proof(ctx, pk, cs, inputs, aux, cudaMemcpyHostToDevice, r_mont, s_mont, check_satisfied, proof_a, proof_b, proof_c);
 }
 
 int32_t bzk_groth16_prove_dev(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const void *d_inputs, const void *d_aux,
                               const bzk_fr *r_mont, const bzk_fr *s_mont, int32_t check_satisfied,
                               bzk_g1_affine *proof_a, bzk_g2_affine *proof_b, bzk_g1_affine *proof_c) {
-    return groth16_prove_impl(ctx, pk, cs, (const bzk_fr *)d_inputs, (const bzk_fr *)d_aux, cudaMemcpyDeviceToDevice, r_mont, s_mont,
-                              check_satisfied, proof_a, proof_b, proof_c);
+    return whole_proof(ctx, pk, cs, (const bzk_fr *)d_inputs, (const bzk_fr *)d_aux, cudaMemcpyDeviceToDevice, r_mont, s_mont,
+                       check_satisfied, proof_a, proof_b, proof_c);
 }
 
 /* milliseconds since the start of the last timed prove call (bzk_ctx_set_timing on) at which: [1] z upload + the three
@@ -535,11 +511,11 @@ int32_t bzk_groth16_params_set_shard(bzk_groth16_params *p, uint32_t rank, uint3
 int32_t bzk_groth16_prove_partial(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const void *inputs, const void *aux,
                                   int32_t witness_on_device, int32_t check_satisfied,
                                   bzk_g1_affine *a_sum, bzk_g1_affine *b1_sum, bzk_g2_affine *b2_sum, bzk_g1_affine *hl_sum) {
-    if (!a_sum || !b1_sum || !b2_sum || !hl_sum) return BZK_ERR_BAD_ARG;
-    const Groth16Partials part{a_sum, b1_sum, hl_sum, b2_sum};
-    return groth16_prove_impl(ctx, pk, cs, (const bzk_fr *)inputs, (const bzk_fr *)aux,
-                              witness_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, nullptr, nullptr, check_satisfied,
-                              nullptr, nullptr, nullptr, &part);
+    if (!ctx || !pk || !cs || !inputs || (cs->num_aux && !aux) || !a_sum || !b1_sum || !b2_sum || !hl_sum) return BZK_ERR_BAD_ARG;
+    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+    BZK_TRY(enqueue_proof(ctx, pk, cs, (const bzk_fr *)inputs, (const bzk_fr *)aux, witness_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                          check_satisfied != 0));
+    return collect(ctx, a_sum, b1_sum, b2_sum, hl_sum);
 }
 
 /* The sharded schedule with the quotient pipeline split over the ranks (include/bzk.h).  begin: z, the evaluation vectors in
@@ -548,22 +524,44 @@ int32_t bzk_groth16_prove_partial(bzk_ctx *ctx, const bzk_groth16_params *pk, co
  * over this rank's slice of the quotient coefficients, then the four partial sums as bzk_groth16_prove_partial returns them. */
 int32_t bzk_groth16_shard_begin(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const void *inputs, const void *aux,
                                 int32_t witness_on_device, uint32_t poly_mask, void *d_evals[3]) {
-    if (!d_evals || poly_mask > 7) return BZK_ERR_BAD_ARG;
-    const Groth16Split sp{1, poly_mask, {(Fr *)d_evals[0], (Fr *)d_evals[1], (Fr *)d_evals[2]}, nullptr};
-    return groth16_prove_impl(ctx, pk, cs, (const bzk_fr *)inputs, (const bzk_fr *)aux,
-                              witness_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, nullptr, nullptr, 0, nullptr, nullptr, nullptr,
-                              nullptr, &sp);
+    if (!ctx || !pk || !cs || !inputs || (cs->num_aux && !aux) || !d_evals || poly_mask > 7) return BZK_ERR_BAD_ARG;
+    Fr *ev[3];
+    for (int s = 0; s < 3; s++) {
+        const bool mine = (poly_mask >> s) & 1;
+        if (mine && !d_evals[s]) return BZK_ERR_BAD_ARG;
+        ev[s] = mine ? (Fr *)d_evals[s] : nullptr;
+    }
+    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+    Slices sl;
+    Stage sg;
+    BZK_TRY(shard_slices(pk, cs, &sl));
+    BZK_TRY(stage_arena(ctx, cs, &sg));
+    BZK_TRY(witness_side(ctx, cs, sg, (const bzk_fr *)inputs, (const bzk_fr *)aux, witness_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                         ev, false));
+    BZK_TRY(witness_sums(ctx, pk, cs, sg, sl));
+    // the pointwise step and the last transform happen on the rank that collects the three vectors (bzk_groth16_h_combine_dev)
+    for (Fr *v : ev)
+        if (v) BZK_TRY(groth16_to_coset_launch(ctx, v, cs->log_m));
+    g16_mark(ctx, 2, ctx->stream);
+    BZK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the caller hands the vectors to its transport next
+    ctx->split_open = true;
+    return BZK_OK;
 }
+/* finish leaves the staging arena alone: the side-stream sums started by begin may still be reading z and the gathered
+ * scalars from it */
 int32_t bzk_groth16_shard_finish(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const void *d_h_shard,
                                  bzk_g1_affine *a_sum, bzk_g1_affine *b1_sum, bzk_g2_affine *b2_sum, bzk_g1_affine *hl_sum) {
-    if (!a_sum || !b1_sum || !b2_sum || !hl_sum) return BZK_ERR_BAD_ARG;
-    const Groth16Partials part{a_sum, b1_sum, hl_sum, b2_sum};
-    const Groth16Split sp{2, 0, {nullptr, nullptr, nullptr}, (const Fr *)d_h_shard};
-    return groth16_prove_impl(ctx, pk, cs, nullptr, nullptr, cudaMemcpyDeviceToDevice, nullptr, nullptr, 0, nullptr, nullptr, nullptr, &part, &sp);
+    if (!ctx || !pk || !cs || !a_sum || !b1_sum || !b2_sum || !hl_sum) return BZK_ERR_BAD_ARG;
+    if (!ctx->split_open || (!d_h_shard && pk->h->n)) return BZK_ERR_BAD_ARG;
+    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+    Slices sl;
+    BZK_TRY(shard_slices(pk, cs, &sl));
+    ctx->split_open = false;
+    BZK_TRY(h_sum(ctx, pk, (const Fr *)d_h_shard, sl.h_n));
+    return collect(ctx, a_sum, b1_sum, b2_sum, hl_sum);
 }
 
-/* bellman `create_proof`'s last lines from the (summed) answers:
- *   A = r*delta1 + alpha1 + a;  B = s*delta2 + beta2 + b2;  C = rs*delta1 + s*alpha1 + r*beta1 + s*a + r*b1 + (h + l) */
+/* the tail of bellman `create_proof` from the (summed) answers, on the host (proof_tail) */
 int32_t bzk_groth16_finalize(const bzk_g1_affine *alpha_g1, const bzk_g1_affine *beta_g1, const bzk_g2_affine *beta_g2,
                              const bzk_g1_affine *delta_g1, const bzk_g2_affine *delta_g2,
                              const bzk_g1_affine *a_sum, const bzk_g1_affine *b1_sum, const bzk_g2_affine *b2_sum, const bzk_g1_affine *hl_sum,
@@ -571,27 +569,12 @@ int32_t bzk_groth16_finalize(const bzk_g1_affine *alpha_g1, const bzk_g1_affine 
     if (!alpha_g1 || !beta_g1 || !beta_g2 || !delta_g1 || !delta_g2 || !a_sum || !b1_sum || !b2_sum || !hl_sum || !r_mont || !s_mont ||
         !proof_a || !proof_b || !proof_c)
         return BZK_ERR_BAD_ARG;
-    Fr r, s;
-    memcpy(r.l, r_mont, 32);
-    memcpy(s.l, s_mont, 32);
-    const Fr rs = (r * s).from_mont(), rc = r.from_mont(), sc = s.from_mont();
-    const G1Affine al = g1_from_img(alpha_g1), be1 = g1_from_img(beta_g1), de1 = g1_from_img(delta_g1), av = g1_from_img(a_sum);
-    G2Xyzz gb = scalar_mul(g2_from_img(delta_g2), sc.l);
-    gb.madd(g2_from_img(beta_g2));
-    gb.madd(g2_from_img(b2_sum));
-    G1Xyzz ga = scalar_mul(de1, rc.l);
-    ga.madd(al);
-    ga.madd(av);
-    G1Xyzz gc = scalar_mul(de1, rs.l);
-    gc.add(scalar_mul(al, sc.l));
-    gc.add(scalar_mul(be1, rc.l));
-    gc.add(scalar_mul(av, sc.l));
-    gc.add(scalar_mul(g1_from_img(b1_sum), rc.l));
-    gc.madd(g1_from_img(hl_sum));
-    g1_to_img(proof_a, ga.to_affine());
-    g2_to_img(proof_b, gb.to_affine());
-    g1_to_img(proof_c, gc.to_affine());
-    return BZK_OK;
+    auto sums = [&](Groth16Partials *p) {
+        *p = Groth16Partials{*a_sum, *b1_sum, *hl_sum, *b2_sum};
+        return (int32_t)BZK_OK;
+    };
+    return proof_tail(from_wire(alpha_g1), from_wire(beta_g1), from_wire(beta_g2), from_wire(delta_g1), from_wire(delta_g2), r_mont, s_mont, sums,
+                      proof_a, proof_b, proof_c);
 }
 
 /* 387-byte bincode image of `Groth16Proof {a, b, c}` (/root/reference/src/zk/groth16/mod.rs:33-38) */

@@ -35,9 +35,9 @@ int32_t random_fr(bzk_ctx *ctx, uint64_t seed, size_t n, Fr *d_out) {
     return BZK_OK;
 }
 int32_t host_g1_add(const bzk_g1_affine *a, const bzk_g1_affine *b, bzk_g1_affine *out) {
-    G1Xyzz acc = G1Xyzz::from_affine(g1_from_image(a));
-    acc.madd(g1_from_image(b));
-    g1_to_image(out, acc.to_affine());
+    G1Xyzz acc = G1Xyzz::from_affine(from_wire(a));
+    acc.madd(from_wire(b));
+    to_wire(out, acc.to_affine());
     return BZK_OK;
 }
 

@@ -29,9 +29,9 @@ int32_t random_g2(bzk_ctx *ctx, uint64_t seed, size_t n, uint8_t *d_out) {
     return BZK_OK;
 }
 int32_t host_g2_add(const bzk_g2_affine *a, const bzk_g2_affine *b, bzk_g2_affine *out) {
-    G2Xyzz acc = G2Xyzz::from_affine(g2_from_image(a));
-    acc.madd(g2_from_image(b));
-    g2_to_image(out, acc.to_affine());
+    G2Xyzz acc = G2Xyzz::from_affine(from_wire(a));
+    acc.madd(from_wire(b));
+    to_wire(out, acc.to_affine());
     return BZK_OK;
 }
 

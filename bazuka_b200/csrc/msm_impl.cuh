@@ -493,58 +493,10 @@ static __global__ void __launch_bounds__(256) k_random_fr(uint64_t seed, size_t 
     store_vec(out + i, splitmix_fr_canonical(seed, i).to_mont());
 }
 
-// wire image (host) <-> Affine<F>
-static G1Affine g1_from_image(const bzk_g1_affine *img) {
-    if (img->infinity) return G1Affine::inf();
-    G1Affine p;
-    memcpy(p.x.l, img->x, 48);
-    memcpy(p.y.l, img->y, 48);
-    return p;
-}
-static void g1_to_image(bzk_g1_affine *img, const G1Affine &p) {
-    memset(img, 0, sizeof *img);
-    if (p.is_inf()) {
-        Fp one = Fp::one();
-        memcpy(img->y, one.l, 48);
-        img->infinity = 1;
-        return;
-    }
-    memcpy(img->x, p.x.l, 48);
-    memcpy(img->y, p.y.l, 48);
-}
-static G2Affine g2_from_image(const bzk_g2_affine *img) {
-    if (img->infinity) return G2Affine::inf();
-    G2Affine p;
-    memcpy(p.x.c0.l, img->x, 48);
-    memcpy(p.x.c1.l, img->x + 6, 48);
-    memcpy(p.y.c0.l, img->y, 48);
-    memcpy(p.y.c1.l, img->y + 6, 48);
-    return p;
-}
-static void g2_to_image(bzk_g2_affine *img, const G2Affine &p) {
-    memset(img, 0, sizeof *img);
-    if (p.is_inf()) {
-        Fp one = Fp::one();
-        memcpy(img->y, one.l, 48);
-        img->infinity = 1;
-        return;
-    }
-    memcpy(img->x, p.x.c0.l, 48);
-    memcpy(img->x + 6, p.x.c1.l, 48);
-    memcpy(img->y, p.y.c0.l, 48);
-    memcpy(img->y + 6, p.y.c1.l, 48);
-}
+// the wire image type of an Affine<F> (converted with from_wire / to_wire, common.cuh)
 template <class F> struct Wire;
-template <> struct Wire<Fp> {
-    typedef bzk_g1_affine image;
-    static void to_image(image *i, const Affine<Fp> &p) { g1_to_image(i, p); }
-    static Affine<Fp> from_image(const image *i) { return g1_from_image(i); }
-};
-template <> struct Wire<Fp2> {
-    typedef bzk_g2_affine image;
-    static void to_image(image *i, const Affine<Fp2> &p) { g2_to_image(i, p); }
-    static Affine<Fp2> from_image(const image *i) { return g2_from_image(i); }
-};
+template <> struct Wire<Fp> { typedef bzk_g1_affine image; };
+template <> struct Wire<Fp2> { typedef bzk_g2_affine image; };
 
 // ---------------------------------------------------------------------------------------------
 // fixed-base table: level t of point i = [2^(bits*t)] P_i, affine.  One thread per base walks the doubling
@@ -815,7 +767,7 @@ static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_
 
 template <class F>
 static void msm_host_finish(const MsmPlan &pl, const Xyzz<F> *h_win, typename Wire<F>::image *out) {
-    if (pl.W == 0) { Wire<F>::to_image(out, Affine<F>::inf()); return; }
+    if (pl.W == 0) { to_wire(out, Affine<F>::inf()); return; }
     // group sum = A + slice * sum_j 2^j T_j  (see k_bucket_slices)
     auto group_sum = [&](uint32_t g) {
         const Xyzz<F> *row = h_win + (size_t)g * (1 + pl.nbits);
@@ -838,7 +790,7 @@ static void msm_host_finish(const MsmPlan &pl, const Xyzz<F> *h_win, typename Wi
         for (uint32_t k = 0; k < pl.c; k++) acc = acc.dbl();
         acc.add(group_sum((uint32_t)w));
     }
-    Wire<F>::to_image(out, acc.to_affine());
+    to_wire(out, acc.to_affine());
 }
 
 template <class F>

@@ -303,7 +303,10 @@ int32_t divide_by_z_launch(bzk_ctx *ctx, Fr *d, uint32_t log_n) {
     return BZK_OK;
 }
 
-// one evaluation vector to the coset: ifft then coset_fft, the first half of the quotient pipeline below
+// one evaluation vector to the coset: ifft then coset_fft, the first half of the quotient pipeline below.  The two
+// transforms run WITHOUT the two permutation passes and the two scaling passes in between: the DIF transform leaves the
+// coefficients bit-reversed, the DIT transform takes them that way, and its first pass applies n^-1 * 7^i to coefficient
+// i on the way in (values identical to the four separate maps)
 int32_t groth16_to_coset_launch(bzk_ctx *ctx, Fr *v, uint32_t log_n) {
     if (log_n > 28 || !v) return BZK_ERR_BAD_ARG;
     BZK_TRY(ensure_tables(ctx, log_n));
@@ -324,25 +327,11 @@ int32_t groth16_h_combine_launch(bzk_ctx *ctx, Fr *a, Fr *b, Fr *c, uint32_t log
     return ntt_launch(ctx, a, log_n, BZK_NTT_ICOSET_FFT);
 }
 
+// the whole quotient pipeline: a <- coefficients of (a*b - c) / Z from the three evaluation vectors
 int32_t groth16_h_launch(bzk_ctx *ctx, Fr *a, Fr *b, Fr *c, uint32_t log_n) {
     if (log_n > 28 || !a || !b || !c) return BZK_ERR_BAD_ARG;
-    const size_t n = (size_t)1 << log_n;
-    Fr *v[3] = {a, b, c};
-    // ifft then coset_fft of each evaluation vector WITHOUT the two permutation passes and the two scaling passes in
-    // between: the DIF transform leaves the coefficients bit-reversed, the DIT transform takes them that way, and
-    // its first pass applies n^-1 * 7^i to coefficient i on the way in (values identical to the four separate maps)
-    BZK_TRY(ensure_tables(ctx, log_n));
-    BZK_TRY(ensure_gpow(ctx));
-    const NttTables &tb = ctx->ntt[log_n];
-    uint32_t e[1] = {log_n};
-    const Fr ninv = Fr::from_u32(2).inv().pow(e, 1);
-    for (int k = 0; k < 3; k++) {
-        BZK_TRY(run_dif(ctx, v[k], log_n, tb.d_inv));
-        BZK_TRY(run_dit_prescaled(ctx, v[k], log_n, tb.d_fwd, ninv, ctx->d_gpow, ctx->d_gpow + kGpowN));
-    }
-    k_h_pointwise<<<div_up(n, 256), 256, 0, ctx->stream>>>(a, b, c, n, host_zinv(log_n));
-    BZK_LAUNCHED(ctx);
-    return ntt_launch(ctx, a, log_n, BZK_NTT_ICOSET_FFT);
+    for (Fr *v : {a, b, c}) BZK_TRY(groth16_to_coset_launch(ctx, v, log_n));
+    return groth16_h_combine_launch(ctx, a, b, c, log_n);
 }
 
 }  // namespace bzk

@@ -209,32 +209,6 @@ static int32_t fault_status(uint32_t f) {
     return f == kNotOnCurve ? BZK_ERR_NOT_ON_CURVE : f == kNotInSubgroup ? BZK_ERR_NOT_IN_SUBGROUP : BZK_ERR_BAD_ENCODING;
 }
 
-// host wire images <-> packed Montgomery points
-static G1Affine packed_g1(const bzk_g1_affine *img) {
-    G1Affine p = G1Affine::inf();
-    if (!img->infinity) { memcpy(p.x.l, img->x, 48); memcpy(p.y.l, img->y, 48); }
-    return p;
-}
-static G2Affine packed_g2(const bzk_g2_affine *img) {
-    G2Affine p = G2Affine::inf();
-    if (!img->infinity) {
-        memcpy(p.x.c0.l, img->x, 48); memcpy(p.x.c1.l, img->x + 6, 48);
-        memcpy(p.y.c0.l, img->y, 48); memcpy(p.y.c1.l, img->y + 6, 48);
-    }
-    return p;
-}
-static void wire_g1(const G1Affine &p, bzk_g1_affine *img) {
-    memset(img, 0, sizeof *img);
-    if (p.is_inf()) { const Fp one = Fp::one(); memcpy(img->y, one.l, 48); img->infinity = 1; return; }
-    memcpy(img->x, p.x.l, 48); memcpy(img->y, p.y.l, 48);
-}
-static void wire_g2(const G2Affine &p, bzk_g2_affine *img) {
-    memset(img, 0, sizeof *img);
-    if (p.is_inf()) { const Fp one = Fp::one(); memcpy(img->y, one.l, 48); img->infinity = 1; return; }
-    memcpy(img->x, p.x.c0.l, 48); memcpy(img->x + 6, p.x.c1.l, 48);
-    memcpy(img->y, p.y.c0.l, 48); memcpy(img->y + 6, p.y.c1.l, 48);
-}
-
 }  // namespace bzk
 
 using namespace bzk;
@@ -353,9 +327,9 @@ int32_t bzk_groth16_params_read(bzk_ctx *ctx, const uint8_t *bytes, size_t len, 
     }
     cudaFree(scratch);
     scratch = nullptr;
-    wire_g1(vk1[0], alpha_g1); wire_g1(vk1[1], beta_g1); wire_g1(vk1[2], delta_g1);
-    wire_g2(vk2[0], beta_g2); wire_g2(vk2[1], gamma_g2); wire_g2(vk2[2], delta_g2);
-    for (uint64_t i = 0; i < n_ic; i++) wire_g1(ic_pts[i], ic + i);
+    to_wire(alpha_g1, vk1[0]); to_wire(beta_g1, vk1[1]); to_wire(delta_g1, vk1[2]);
+    to_wire(beta_g2, vk2[0]); to_wire(gamma_g2, vk2[1]); to_wire(delta_g2, vk2[2]);
+    for (uint64_t i = 0; i < n_ic; i++) to_wire(ic + i, ic_pts[i]);
     st = bzk_groth16_params_create(ctx, alpha_g1, beta_g1, beta_g2, delta_g1, delta_g2, g1v[0], g1v[1], g1v[2], g1v[3], b2, out);
     if (st != BZK_OK) release();
     return st;
@@ -386,9 +360,9 @@ int32_t bzk_groth16_params_write(bzk_ctx *ctx, const bzk_groth16_params *params,
 
     // the verifying key's points go through the same kernels from a scratch block
     std::vector<G1Affine> vk1(3 + n_ic);
-    G2Affine vk2[3] = {params->beta_g2, packed_g2(gamma_g2), params->delta_g2};
+    G2Affine vk2[3] = {params->beta_g2, from_wire(gamma_g2), params->delta_g2};
     vk1[0] = params->alpha_g1; vk1[1] = params->beta_g1; vk1[2] = params->delta_g1;
-    for (size_t i = 0; i < n_ic; i++) vk1[3 + i] = packed_g1(ic + i);
+    for (size_t i = 0; i < n_ic; i++) vk1[3 + i] = from_wire(ic + i);
     void *scratch = nullptr;
     BZK_CUDA(ctx, cudaMalloc(&scratch, vk1.size() * sizeof(G1Affine) + sizeof vk2 + 256));
     G1Affine *d_vk1 = (G1Affine *)scratch;

@@ -35,24 +35,9 @@ struct bzk_groth16_pvk {
 
 namespace {
 
-G1Affine img_g1(const bzk_g1_affine *img) {
-    if (img->infinity) return G1Affine::inf();
-    G1Affine p;
-    memcpy(p.x.l, img->x, 48);
-    memcpy(p.y.l, img->y, 48);
-    return p;
-}
-G2Affine img_g2(const bzk_g2_affine *img) {
-    if (img->infinity) return G2Affine::inf();
-    G2Affine p;
-    memcpy(p.x.c0.l, img->x, 48); memcpy(p.x.c1.l, img->x + 6, 48);
-    memcpy(p.y.c0.l, img->y, 48); memcpy(p.y.c1.l, img->y + 6, 48);
-    return p;
-}
-bool on_curve_g1(const G1Affine &p) { return p.is_inf() || p.y.sqr() == p.x.sqr() * p.x + Fp::from_u32(4); }
-bool on_curve_g2(const G2Affine &p) {
-    Fp four = Fp::from_u32(4);
-    return p.is_inf() || p.y.sqr() == p.x.sqr() * p.x + Fp2{four, four};
+// a proof's three points lie on their curves (the identity counts as on them)
+bool on_curves(const G1Affine &A, const G2Affine &B, const G1Affine &C) {
+    return (A.is_inf() || on_curve(A)) && (B.is_inf() || on_curve(B)) && (C.is_inf() || on_curve(C));
 }
 bzk_g1_affine g1_at(const uint8_t *p) { bzk_g1_affine g; memset(&g, 0, sizeof g); memcpy(&g, p, 97); return g; }
 bzk_g2_affine g2_at(const uint8_t *p) { bzk_g2_affine g; memset(&g, 0, sizeof g); memcpy(&g, p, 193); return g; }
@@ -86,7 +71,7 @@ G1Affine input_accumulator(const bzk_groth16_pvk *k, const bzk_fr *inputs, size_
 }
 
 int32_t verify_one(const bzk_groth16_pvk *k, const bzk_fr *inputs, size_t n, const G1Affine &A, const G2Affine &B, const G1Affine &C) {
-    if (!on_curve_g1(A) || !on_curve_g1(C) || !on_curve_g2(B)) return 0;
+    if (!on_curves(A, B, C)) return 0;
     G2Lines bl;
     compute_lines(B, bl);
     const MillerPair pairs[3] = {{A, &bl}, {input_accumulator(k, inputs, n).neg(), &k->gamma_lines}, {C.neg(), &k->delta_lines}};
@@ -106,8 +91,8 @@ int32_t parse_vk(const uint8_t *vk, size_t vk_len, bzk_groth16_pvk **out) {
     memcpy(&n_ic, vk + off, 8); off += 8;
     if (n_ic == 0 || n_ic > 4096 || vk_len != off + 97 * n_ic) return BZK_ERR_BAD_ARG;
     std::vector<G1Affine> ic(n_ic);
-    for (uint64_t i = 0; i < n_ic; i++) { bzk_g1_affine g = g1_at(vk + off + 97 * i); ic[i] = img_g1(&g); }
-    bzk_groth16_pvk *k = prepare(img_g1(&alpha), img_g2(&beta), img_g2(&gamma), img_g2(&delta), std::move(ic));
+    for (uint64_t i = 0; i < n_ic; i++) { bzk_g1_affine g = g1_at(vk + off + 97 * i); ic[i] = from_wire(&g); }
+    bzk_groth16_pvk *k = prepare(from_wire(&alpha), from_wire(&beta), from_wire(&gamma), from_wire(&delta), std::move(ic));
     if (!k) return BZK_ERR_OOM;
     k->image.assign(vk, vk + vk_len);
     *out = k;
@@ -225,8 +210,8 @@ int32_t bzk_groth16_pvk_create(const bzk_g1_affine *alpha_g1, const bzk_g2_affin
                                const bzk_g2_affine *delta_g2, const bzk_g1_affine *ic, size_t n_ic, bzk_groth16_pvk **out) {
     if (!alpha_g1 || !beta_g2 || !gamma_g2 || !delta_g2 || !ic || !n_ic || !out) return BZK_ERR_BAD_ARG;
     std::vector<G1Affine> icv(n_ic);
-    for (size_t i = 0; i < n_ic; i++) icv[i] = img_g1(&ic[i]);
-    bzk_groth16_pvk *k = prepare(img_g1(alpha_g1), img_g2(beta_g2), img_g2(gamma_g2), img_g2(delta_g2), std::move(icv));
+    for (size_t i = 0; i < n_ic; i++) icv[i] = from_wire(&ic[i]);
+    bzk_groth16_pvk *k = prepare(from_wire(alpha_g1), from_wire(beta_g2), from_wire(gamma_g2), from_wire(delta_g2), std::move(icv));
     if (!k) return BZK_ERR_OOM;
     *out = k;
     return BZK_OK;
@@ -244,7 +229,7 @@ int32_t bzk_groth16_pvk_free(bzk_groth16_pvk *k) {
 int32_t bzk_groth16_verify_prepared(const bzk_groth16_pvk *k, const bzk_fr *public_inputs, size_t n_inputs,
                                     const bzk_g1_affine *proof_a, const bzk_g2_affine *proof_b, const bzk_g1_affine *proof_c) {
     if (!k || !proof_a || !proof_b || !proof_c || k->ic.size() != n_inputs + 1 || (n_inputs && !public_inputs)) return BZK_ERR_BAD_ARG;
-    return verify_one(k, public_inputs, n_inputs, img_g1(proof_a), img_g2(proof_b), img_g1(proof_c));
+    return verify_one(k, public_inputs, n_inputs, from_wire(proof_a), from_wire(proof_b), from_wire(proof_c));
 }
 
 int32_t bzk_groth16_verify(const bzk_g1_affine *alpha_g1, const bzk_g2_affine *beta_g2, const bzk_g2_affine *gamma_g2,
@@ -265,7 +250,7 @@ int32_t bzk_groth16_verify(const bzk_g1_affine *alpha_g1, const bzk_g2_affine *b
     int32_t st = BZK_OK;
     auto k = cache().get(img.data(), img.size(), &st);
     if (!k) return st;
-    return verify_one(k.get(), public_inputs, n_inputs, img_g1(proof_a), img_g2(proof_b), img_g1(proof_c));
+    return verify_one(k.get(), public_inputs, n_inputs, from_wire(proof_a), from_wire(proof_b), from_wire(proof_c));
 }
 
 /* `check_proof` on the reference's byte images (/root/reference/src/zk/mod.rs:157-193): vk = bincode
@@ -279,7 +264,7 @@ int32_t bzk_groth16_verify_bytes(const uint8_t *vk, size_t vk_len, const bzk_fr 
     if (k->ic.size() != n_inputs + 1 || (n_inputs && !public_inputs)) return BZK_ERR_BAD_ARG;
     const bzk_g1_affine a = g1_at(proof387), c = g1_at(proof387 + 290);
     const bzk_g2_affine b = g2_at(proof387 + 97);
-    return verify_one(k.get(), public_inputs, n_inputs, img_g1(&a), img_g2(&b), img_g1(&c));
+    return verify_one(k.get(), public_inputs, n_inputs, from_wire(&a), from_wire(&b), from_wire(&c));
 }
 
 /* m proofs under one key.  inputs: m rows of n_inputs Montgomery scalars; proofs: m x 387 bytes; seed: randomness for
@@ -300,7 +285,7 @@ int32_t bzk_groth16_verify_batch(const bzk_groth16_pvk *k, const bzk_fr *public_
         const uint8_t *p = proofs387 + 387 * j;
         const bzk_g1_affine a = g1_at(p), c = g1_at(p + 290);
         const bzk_g2_affine b = g2_at(p + 97);
-        A[j] = img_g1(&a); B[j] = img_g2(&b); C[j] = img_g1(&c);
+        A[j] = from_wire(&a); B[j] = from_wire(&b); C[j] = from_wire(&c);
     }
     std::vector<Fr> r;
     derive_multipliers(seed, m, r);
@@ -313,7 +298,7 @@ int32_t bzk_groth16_verify_batch(const bzk_groth16_pvk *k, const bzk_fr *public_
         Fp12 f = f12_one();
         G1Xyzz cs = G1Xyzz::inf();
         for (size_t j = lo; j < hi; j++) {
-            if (!on_curve_g1(A[j]) || !on_curve_g1(C[j]) || !on_curve_g2(B[j])) { bad[t] = 1; continue; }
+            if (!on_curves(A[j], B[j], C[j])) { bad[t] = 1; continue; }
             G2Lines bl;
             compute_lines(B[j], bl);
             const MillerPair p{small_msm(&A[j], &r[j], 1, 127).to_affine(), &bl};

@@ -15,10 +15,12 @@ production boundary: `MpnWork` in, `ZkProof::Groth16` out, /root/reference/src/m
                 (params, r, s, witness))
 """
 import ctypes as ct
+import os
 
 import numpy as np
 
-from .api import Context, G1_BYTES, G2_BYTES, _host_ptr, NTT_IFFT
+from . import _lib
+from .api import Context, G1_BYTES, G2_BYTES, _dev_ptr, _host_ptr, NTT_IFFT
 
 
 def _mont_fp_bytes(x):
@@ -135,7 +137,6 @@ def _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels=None):
 def _with_tables(pk, table_levels):
     """the fixed-base table policy of proving_key_from_host"""
     if table_levels is None:
-        import os
         lv = os.environ.get("BZK_TABLE_LEVELS")   # development override: 1 = no tables
         table_levels = int(lv) if lv else 0
     if table_levels != 1:
@@ -148,7 +149,6 @@ def _with_tables(pk, table_levels):
 # ------------------------------------------------------------------------------------------------
 def _file_bytes(src):
     """a path (memory-mapped, never loaded whole) or a bytes-like object -> uint8 array"""
-    import os
     if isinstance(src, (str, os.PathLike)):
         if os.path.getsize(src) == 0:
             return np.zeros(0, dtype=np.uint8)
@@ -163,7 +163,6 @@ PARAMS_FILE_INFO = np.dtype([(k, np.uint64) for k in ("n_ic", "n_h", "n_l", "n_a
 
 def parameters_info(src):
     """the header of a bellman `Parameters` file (bzk_groth16_params_file_info): point counts and the byte count they imply"""
-    from . import _lib
     lib = _lib.load()
     buf = _file_bytes(src)
     out = np.zeros(1, dtype=PARAMS_FILE_INFO)
@@ -235,21 +234,32 @@ class Prover:
         except Exception:
             pass
 
-    def prove(self, pk: ProvingKey, inputs, aux, r, s, check_satisfied=True):
-        """inputs [num_inputs,4] (inputs[0] = R(1)), aux [num_aux,4], r/s [4] — Montgomery.
-        Returns (proof_bytes[387], (a[104], b[200], c[104]))."""
+    def _host_witness(self, inputs, aux):
         inputs = np.ascontiguousarray(inputs, dtype=np.uint64).reshape(-1, 4)
         aux = np.ascontiguousarray(aux, dtype=np.uint64).reshape(-1, 4)
         assert len(inputs) == self.r1cs.num_inputs and len(aux) == self.r1cs.num_aux
+        return inputs, aux
+
+    def prove(self, pk: ProvingKey, inputs, aux, r, s, check_satisfied=True):
+        """inputs [num_inputs,4] (inputs[0] = R(1)), aux [num_aux,4], r/s [4] — Montgomery.
+        Returns (proof_bytes[387], (a[104], b[200], c[104]))."""
+        inputs, aux = self._host_witness(inputs, aux)
+        return self._prove(self.ctx._l.bzk_groth16_prove, pk, _host_ptr(inputs), _host_ptr(aux), r, s, check_satisfied)
+
+    def prove_dev(self, pk: ProvingKey, d_inputs, d_aux, r, s, check_satisfied=True):
+        """`prove` with the witness already resident: d_inputs [num_inputs,4], d_aux [num_aux,4] CUDA int64
+        tensors of Montgomery images (e.g. written by mpn.gpu_witness)."""
+        assert d_inputs.numel() == 4 * self.r1cs.num_inputs and d_aux.numel() == 4 * self.r1cs.num_aux
+        return self._prove(self.ctx._l.bzk_groth16_prove_dev, pk, _dev_ptr(d_inputs), _dev_ptr(d_aux), r, s, check_satisfied)
+
+    def _prove(self, entry, pk, p_inputs, p_aux, r, s, check_satisfied):
         r = np.ascontiguousarray(r, dtype=np.uint64).reshape(4)
         s = np.ascontiguousarray(s, dtype=np.uint64).reshape(4)
         pa, pb, pc = np.zeros(G1_BYTES, np.uint8), np.zeros(G2_BYTES, np.uint8), np.zeros(G1_BYTES, np.uint8)
         c = self.ctx
-        c._check(c._l.bzk_groth16_prove(c._h, pk._h, self._h, _host_ptr(inputs), _host_ptr(aux), _host_ptr(r), _host_ptr(s),
-                                         int(check_satisfied), _host_ptr(pa), _host_ptr(pb), _host_ptr(pc)))
-        blob = np.zeros(387, np.uint8)
-        c._check(c._l.bzk_groth16_proof_bytes(_host_ptr(pa), _host_ptr(pb), _host_ptr(pc), _host_ptr(blob)))
-        return blob, (pa, pb, pc)
+        c._check(entry(c._h, pk._h, self._h, p_inputs, p_aux, _host_ptr(r), _host_ptr(s), int(check_satisfied),
+                       _host_ptr(pa), _host_ptr(pb), _host_ptr(pc)))
+        return _proof_blob(c._l, pa, pb, pc), (pa, pb, pc)
 
     STAGES = ("z_spmv_done", "quotient_ntts_done", "h_msm_done", "l_msm_done", "a_msm_done", "b_g1_msm_done", "b_g2_msm_done")
 
@@ -260,29 +270,27 @@ class Prover:
         ok = self.ctx._l.bzk_groth16_stage_ms(self.ctx._h, _host_ptr(out))
         return {k: float(out[i + 1]) for i, k in enumerate(self.STAGES)} if ok == 1 else None
 
+    def _partials(self, entry, spk, *args):
+        """entry(ctx, spk, r1cs, *args, a_sum, b1_sum, b2_sum, hl_sum) -> the four partial sums (a, b_g1, b_g2, h+l wire images)"""
+        sums = np.zeros(G1_BYTES, np.uint8), np.zeros(G1_BYTES, np.uint8), np.zeros(G2_BYTES, np.uint8), np.zeros(G1_BYTES, np.uint8)
+        c = self.ctx
+        c._check(entry(c._h, spk._h, self._h, *args, *[_host_ptr(x) for x in sums]))
+        return sums
+
     def prove_partial(self, spk: ProvingKey, inputs, aux, check_satisfied=True):
         """this rank's four partial sums (a, b_g1, b_g2, h+l wire images) under the base-sharded key `spk`
         (shard_proving_key).  inputs/aux: host arrays, or CUDA tensors for a resident witness."""
-        c = self.ctx
         on_dev = hasattr(inputs, "is_cuda")
         if on_dev:
-            from .api import _dev_ptr
             pi, pa_ = _dev_ptr(inputs), _dev_ptr(aux)
         else:
-            inputs = np.ascontiguousarray(inputs, dtype=np.uint64).reshape(-1, 4)
-            aux = np.ascontiguousarray(aux, dtype=np.uint64).reshape(-1, 4)
-            assert len(inputs) == self.r1cs.num_inputs and len(aux) == self.r1cs.num_aux
+            inputs, aux = self._host_witness(inputs, aux)
             pi, pa_ = _host_ptr(inputs), _host_ptr(aux)
-        a_sum, b1_sum, hl_sum, b2_sum = np.zeros(G1_BYTES, np.uint8), np.zeros(G1_BYTES, np.uint8), np.zeros(G1_BYTES, np.uint8), np.zeros(G2_BYTES, np.uint8)
-        c._check(c._l.bzk_groth16_prove_partial(c._h, spk._h, self._h, pi, pa_, int(on_dev), int(check_satisfied),
-                                                 _host_ptr(a_sum), _host_ptr(b1_sum), _host_ptr(b2_sum), _host_ptr(hl_sum)))
-        return a_sum, b1_sum, b2_sum, hl_sum
+        return self._partials(self.ctx._l.bzk_groth16_prove_partial, spk, pi, pa_, int(on_dev), int(check_satisfied))
 
     def shard_begin(self, spk: ProvingKey, d_inputs, d_aux, evals):
         """first half of the split sharded schedule: evals = [tensor | None] * 3 — the evaluation vectors (a, b, c) this rank owns,
         as CUDA int64 tensors [2^log_m, 4] that receive them on the coset; the four witness sums start on their streams."""
-        import ctypes as ct
-        from .api import _dev_ptr
         c = self.ctx
         ptrs = (ct.c_void_p * 3)(*[_dev_ptr(e) if e is not None else None for e in evals])
         mask = sum(1 << k for k, e in enumerate(evals) if e is not None)
@@ -290,33 +298,12 @@ class Prover:
 
     def h_combine(self, d_a, d_b, d_c):
         """(a*b - c)/Z from the three vectors on the coset, back to coefficients: d_a <- h"""
-        from .api import _dev_ptr
         c = self.ctx
         c._check(c._l.bzk_groth16_h_combine_dev(c._h, _dev_ptr(d_a), _dev_ptr(d_b), _dev_ptr(d_c), self.log_m))
 
     def shard_finish(self, spk: ProvingKey, d_h_shard):
         """second half: the h sum over this rank's slice of the quotient -> (a, b_g1, b_g2, h+l) partial sums"""
-        from .api import _dev_ptr
-        c = self.ctx
-        a_sum, b1_sum, hl_sum, b2_sum = np.zeros(G1_BYTES, np.uint8), np.zeros(G1_BYTES, np.uint8), np.zeros(G1_BYTES, np.uint8), np.zeros(G2_BYTES, np.uint8)
-        c._check(c._l.bzk_groth16_shard_finish(c._h, spk._h, self._h, _dev_ptr(d_h_shard) if d_h_shard is not None else None,
-                                                _host_ptr(a_sum), _host_ptr(b1_sum), _host_ptr(b2_sum), _host_ptr(hl_sum)))
-        return a_sum, b1_sum, b2_sum, hl_sum
-
-    def prove_dev(self, pk: ProvingKey, d_inputs, d_aux, r, s, check_satisfied=True):
-        """`prove` with the witness already resident: d_inputs [num_inputs,4], d_aux [num_aux,4] CUDA int64
-        tensors of Montgomery images (e.g. written by mpn.gpu_witness)."""
-        from .api import _dev_ptr
-        assert d_inputs.numel() == 4 * self.r1cs.num_inputs and d_aux.numel() == 4 * self.r1cs.num_aux
-        r = np.ascontiguousarray(r, dtype=np.uint64).reshape(4)
-        s = np.ascontiguousarray(s, dtype=np.uint64).reshape(4)
-        pa, pb, pc = np.zeros(G1_BYTES, np.uint8), np.zeros(G2_BYTES, np.uint8), np.zeros(G1_BYTES, np.uint8)
-        c = self.ctx
-        c._check(c._l.bzk_groth16_prove_dev(c._h, pk._h, self._h, _dev_ptr(d_inputs), _dev_ptr(d_aux), _host_ptr(r), _host_ptr(s),
-                                             int(check_satisfied), _host_ptr(pa), _host_ptr(pb), _host_ptr(pc)))
-        blob = np.zeros(387, np.uint8)
-        c._check(c._l.bzk_groth16_proof_bytes(_host_ptr(pa), _host_ptr(pb), _host_ptr(pc), _host_ptr(blob)))
-        return blob, (pa, pb, pc)
+        return self._partials(self.ctx._l.bzk_groth16_shard_finish, spk, _dev_ptr(d_h_shard) if d_h_shard is not None else None)
 
 
 def shard_proving_key(ctx, pk: ProvingKey, log_m, rank, world):
@@ -342,7 +329,6 @@ def shard_proving_key(ctx, pk: ProvingKey, log_m, rank, world):
 
 def finalize(vk, partials, r, s):
     """tail of bellman `create_proof` from the summed answers (a, b_g1, b_g2, h+l) -> (blob[387], points)."""
-    from . import _lib
     lib = _lib.load()
     pts = [np.ascontiguousarray(vk[k], dtype=np.uint8) for k in ("alpha_g1", "beta_g1", "beta_g2", "delta_g1", "delta_g2")]
     a_sum, b1_sum, b2_sum, hl_sum = (np.ascontiguousarray(x, dtype=np.uint8) for x in partials)
@@ -353,9 +339,16 @@ def finalize(vk, partials, r, s):
                                   _host_ptr(r), _host_ptr(s), _host_ptr(pa), _host_ptr(pb), _host_ptr(pc))
     if st != 0:
         raise _lib.BzkError(st, "groth16_finalize")
+    return _proof_blob(lib, pa, pb, pc), (pa, pb, pc)
+
+
+def _proof_blob(lib, pa, pb, pc):
+    """the 387-byte bincode image of `Groth16Proof {a, b, c}` (bzk_groth16_proof_bytes)"""
     blob = np.zeros(387, np.uint8)
-    lib.bzk_groth16_proof_bytes(_host_ptr(pa), _host_ptr(pb), _host_ptr(pc), _host_ptr(blob))
-    return blob, (pa, pb, pc)
+    st = lib.bzk_groth16_proof_bytes(_host_ptr(pa), _host_ptr(pb), _host_ptr(pc), _host_ptr(blob))
+    if st != 0:
+        raise _lib.BzkError(st, "groth16_proof_bytes")
+    return blob
 
 
 def allgather_partials(partials, group=None, device="cpu"):
@@ -434,7 +427,6 @@ def verify(vk, public_inputs, proof_points):
     """`groth16_verify` (/root/reference/src/zk/groth16/mod.rs:67-121): vk = dict of wire images
     (alpha_g1, beta_g2, gamma_g2, delta_g2, ic[n+1]), public_inputs [n,4] Montgomery (without ONE),
     proof_points = (a[104], b[200], c[104]).  Host pairing in libbzk; no GPU needed."""
-    from . import _lib
     lib = _lib.load()
     ic = np.ascontiguousarray(vk["ic"], dtype=np.uint8).reshape(-1, G1_BYTES)
     pub = np.ascontiguousarray(public_inputs, dtype=np.uint64).reshape(-1, 4)
@@ -458,7 +450,6 @@ def vk_to_bincode(vk):
 
 def verify_bytes(vk_blob, public_inputs, proof387):
     """`check_proof` on the reference's byte images."""
-    from . import _lib
     lib = _lib.load()
     as_u8 = lambda b: np.frombuffer(bytes(b), dtype=np.uint8) if isinstance(b, (bytes, bytearray, memoryview)) else np.ascontiguousarray(b, dtype=np.uint8)
     vk_blob, proof387 = as_u8(vk_blob), as_u8(proof387)
@@ -632,7 +623,6 @@ class PreparedVerifyingKey:
     coefficients of gamma / delta are computed once.  `vk`: the 878+97n-byte bincode image or a dict of wire images."""
 
     def __init__(self, vk):
-        from . import _lib
         self._l = _lib.load()
         blob = np.ascontiguousarray(vk_to_bincode(vk) if isinstance(vk, dict) else vk, dtype=np.uint8)
         h = ct.c_void_p()
@@ -660,7 +650,6 @@ class PreparedVerifyingKey:
         return self.verify_points(public_inputs, (a, b, c))
 
     def verify_points(self, public_inputs, proof_points):
-        from . import _lib
         pub = np.ascontiguousarray(public_inputs, dtype=np.uint64).reshape(-1, 4)
         a, b, c = (np.ascontiguousarray(x, dtype=np.uint8) for x in proof_points)
         st = self._l.bzk_groth16_verify_prepared(self._h, _host_ptr(pub), len(pub), _host_ptr(a), _host_ptr(b), _host_ptr(c))
@@ -670,8 +659,6 @@ class PreparedVerifyingKey:
 
     def verify_batch_gpu(self, ctx, public_inputs, proofs387, seed=None):
         """verify_batch with the per-proof Miller loops on the GPU (bzk_groth16_verify_batch_dev): same verdicts."""
-        import os
-        from . import _lib
         proofs = np.ascontiguousarray(proofs387, dtype=np.uint8).reshape(-1, 387)
         m = len(proofs)
         if m == 0:
@@ -688,8 +675,6 @@ class PreparedVerifyingKey:
     def verify_batch(self, public_inputs, proofs387, seed=None, threads=0):
         """public_inputs [m, n, 4] Montgomery, proofs387 [m, 387] -> (all_ok, ok_each[m]).  One final exponentiation for
         the batch (random linear combination with 127-bit multipliers from `seed`, default os.urandom)."""
-        import os
-        from . import _lib
         pub = np.ascontiguousarray(public_inputs, dtype=np.uint64)
         proofs = np.ascontiguousarray(proofs387, dtype=np.uint8).reshape(-1, 387)
         m = len(proofs)

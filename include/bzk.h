@@ -281,7 +281,7 @@ int32_t bzk_groth16_prove_partial(bzk_ctx *ctx, const bzk_groth16_params *params
  * owned by rank s mod world, which computes it from z and takes it to the coset (ifft, coset_fft); the owners send their
  * vectors to rank 3 mod world, which forms (a*b - c)/Z and the quotient's coefficients (bzk_groth16_h_combine_dev: a <- h) and
  * hands rank k the slice [(m-1)k/world, (m-1)(k+1)/world) of them.  The transport between GPUs is the caller's
- * (bazuka_b200.groth16.prove_sharded_split uses NCCL point-to-point through torch.distributed).
+ * (bazuka_b200.groth16.SplitShardedProver uses NCCL point-to-point through torch.distributed).
  *   bzk_groth16_shard_begin   z, the vectors in poly_mask into the caller's device buffers d_evals[s] (2^log_m scalars each),
  *                             and the l / a / b_g1 / b_g2 partial sums enqueued — they keep the GPU busy during the exchange
  *   bzk_groth16_shard_finish  the h partial sum over d_h_shard, then the four partial sums of bzk_groth16_prove_partial */
