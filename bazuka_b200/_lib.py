@@ -79,6 +79,8 @@ SIGNATURES = {
     "bzk_r1cs_upload": (_i32, [_vp, _u64, _u64, _u64] + [_vp] * 9 + [ct.POINTER(_vp)]),
     "bzk_r1cs_free": (_i32, [_vp, _vp]),
     "bzk_r1cs_shape": (_i32, [_vp, _vp]),
+    "bzk_r1cs_upload_blocked": (_i32, [_vp] + [_u64] * 8 + [_vp] * 3 + [ct.POINTER(_vp)]),
+    "bzk_r1cs_columns_dev": (_i32, [_vp, _vp, _u32, _vp, _vp]),
     "bzk_groth16_params_create": (_i32, [_vp] * 11 + [ct.POINTER(_vp)]),
     "bzk_groth16_params_free": (_i32, [_vp, _vp]),
     "bzk_groth16_prove": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
@@ -115,6 +117,8 @@ SIGNATURES = {
     "bzk_mpn_circuit_free": (_i32, [_vp]),
     "bzk_mpn_circuit_shape": (_i32, [_vp, _vp]),
     "bzk_mpn_circuit_matrix": (_i32, [_vp, _u32, _vp, _vp, _vp]),
+    "bzk_mpn_update_circuit_compile_blocked": (_i32, [_u32, _u32, _u32, _vp, _sz, _vp, ct.POINTER(_vp)]),
+    "bzk_mpn_circuit_blocks": (_i32, [_vp, _vp]),
     "bzk_mpn_circuit_program": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bzk_mpn_state_clone": (_i32, [_vp, ct.POINTER(_vp)]),
     "bzk_mpn_state_info": (_i32, [_vp, _vp, ct.POINTER(_u64), ct.POINTER(_u64), ct.POINTER(_u64)]),
@@ -161,6 +165,8 @@ SIGNATURES = {
     "bzk_csr_spmv_dev": (_i32, [_vp, _vp, _vp, _vp, _u64, _vp, _vp]),
     "bzk_g1_fixed_base_mul_dev": (_i32, [_vp, _vp, _vp, _sz, _vp]),
     "bzk_g2_fixed_base_mul_dev": (_i32, [_vp, _vp, _vp, _sz, _vp]),
+    "bzk_g1_bases_fixed_base_mul": (_i32, [_vp, _vp, _vp, _sz, ct.POINTER(_vp)]),
+    "bzk_g2_bases_fixed_base_mul": (_i32, [_vp, _vp, _vp, _sz, ct.POINTER(_vp)]),
     "bzk_fr_binop_dev": (_i32, [_vp, _i32, _vp, _vp, _vp, _sz]),
     "bzk_fp_mul_dev": (_i32, [_vp, _vp, _vp, _vp, _sz]),
 }

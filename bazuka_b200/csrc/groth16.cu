@@ -15,6 +15,7 @@
 // kernel instead of re-synthesising the circuit per proof; density trackers become index lists
 // built once at upload; all vectors stay in HBM between stages.
 #include "common.cuh"
+#include "r1cs_blocked.cuh"
 #include <algorithm>
 #include <future>
 
@@ -34,14 +35,34 @@ struct DevCsr {
     Fr *val = nullptr;
     uint64_t nnz = 0;
 };
+// a HostColList on the device
+struct DevColList {
+    uint64_t n = 0;
+    uint32_t *col = nullptr, *row = nullptr;
+    uint64_t *ptr = nullptr;
+    Fr *val = nullptr;
+};
+// a HostBlockedT on the device: one side's transposed pieces, for bzk_r1cs_columns_dev
+struct DevBlockedT {
+    uint64_t span = 0;
+    uint64_t *s_ptr = nullptr;
+    uint32_t *s_row = nullptr;
+    Fr *s_val = nullptr;
+    DevColList shared, fixed;
+};
 }  // namespace bzk
 
+// m[s] holds the stored rows: all ncons of them, or, for a blocked handle, head | template | tail (r1cs_blocked.cuh)
 struct bzk_r1cs {
     uint64_t num_inputs = 0, num_aux = 0, ncons = 0;
     uint32_t log_m = 0;
     bzk::DevCsr m[3];
     uint32_t *d_a_idx = nullptr, *d_b_idx = nullptr;  // indices into z for the A / B sums
     uint64_t a_len = 0, b_len = 0;
+    bool blocked = false;
+    bzk::BlockedShape shape;
+    bzk::DevBlockedT t[3];
+    std::vector<void *> extra;  // the device arrays of t[]
 };
 
 namespace bzk {
@@ -81,6 +102,49 @@ __global__ void __launch_bounds__(64) k_fixed_base_g2(G2Affine base, const Fr *_
     store_g2_image(out + i * 200, scalar_mul(base, k.l).to_affine());
 }
 
+// one thread per logical row of a blocked R1CS; the template rows stay in L2 while the copies read them
+__global__ void __launch_bounds__(256) k_blocked_spmv(BlockedShape b, const uint64_t *__restrict__ rowptr, const uint32_t *__restrict__ col,
+                                                      const Fr *__restrict__ val, uint64_t nrows, const Fr *__restrict__ z, Fr *__restrict__ out) {
+    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= nrows) return;
+    store_vec(out + r, blocked_row_dot(b, rowptr, col, val, r, z));
+}
+// the transposed product's passes (r1cs_blocked.cuh): every column's slot part (0 below var_lo), the per-row sums over the
+// copies, then the shared and the head / tail lists added to the columns they name
+__global__ void __launch_bounds__(256) k_blocked_slot_cols(BlockedShape b, uint64_t span, const uint64_t *__restrict__ s_ptr,
+                                                           const uint32_t *__restrict__ s_row, const Fr *__restrict__ s_val,
+                                                           const Fr *__restrict__ lag, uint64_t nv, Fr *__restrict__ out) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= nv) return;
+    store_vec(out + j, blocked_slot_column(b, span, s_ptr, s_row, s_val, lag, j));
+}
+__global__ void __launch_bounds__(256) k_blocked_rowsum(BlockedShape b, const Fr *__restrict__ lag, Fr *__restrict__ sums) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= b.tmpl_rows) return;
+    store_vec(sums + t, blocked_tmpl_rowsum(b, lag, t));
+}
+__global__ void __launch_bounds__(256) k_col_list_add(uint64_t n, const uint32_t *__restrict__ col, const uint64_t *__restrict__ ptr,
+                                                      const uint32_t *__restrict__ row, const Fr *__restrict__ val, const Fr *__restrict__ w,
+                                                      Fr *__restrict__ out) {
+    const uint64_t u = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (u >= n) return;
+    Fr *o = out + col[u];
+    store_vec(o, load_vec(o) + col_list_dot(ptr, row, val, w, u));
+}
+// k_fixed_base_g1 / _g2 with the packed point stored into a resident vector
+__global__ void __launch_bounds__(128) k_fixed_base_packed_g1(G1Affine base, const Fr *__restrict__ k_mont, size_t n, G1Affine *__restrict__ out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fr k = load_vec(k_mont + i).from_mont();
+    store_vec(out + i, scalar_mul(base, k.l).to_affine());
+}
+__global__ void __launch_bounds__(64) k_fixed_base_packed_g2(G2Affine base, const Fr *__restrict__ k_mont, size_t n, G2Affine *__restrict__ out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fr k = load_vec(k_mont + i).from_mont();
+    store_vec(out + i, scalar_mul(base, k.l).to_affine());
+}
+
 static int32_t upload_csr(bzk_ctx *ctx, DevCsr &d, uint64_t nrows, const uint64_t *rp, const uint32_t *col, const bzk_fr *val) {
     d.nnz = rp[nrows];
     BZK_CUDA(ctx, cudaMalloc(&d.rowptr, (nrows + 1) * sizeof(uint64_t)));
@@ -91,8 +155,32 @@ static int32_t upload_csr(bzk_ctx *ctx, DevCsr &d, uint64_t nrows, const uint64_
     BZK_CUDA(ctx, cudaMemcpyAsync(d.val, val, d.nnz * sizeof(Fr), cudaMemcpyHostToDevice, ctx->stream));
     return BZK_OK;
 }
+// a host vector copied into a new device array that the handle frees
+template <class T>
+static int32_t upload_extra(bzk_ctx *ctx, bzk_r1cs *r, const std::vector<T> &v, T **out) {
+    BZK_CUDA(ctx, cudaMalloc(out, (v.size() ? v.size() : 1) * sizeof(T)));
+    r->extra.push_back(*out);
+    BZK_CUDA(ctx, cudaMemcpyAsync(*out, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+    return BZK_OK;
+}
+static int32_t upload_col_list(bzk_ctx *ctx, bzk_r1cs *r, const HostColList &h, DevColList &d) {
+    d.n = h.col.size();
+    BZK_TRY(upload_extra(ctx, r, h.col, &d.col));
+    BZK_TRY(upload_extra(ctx, r, h.ptr, &d.ptr));
+    BZK_TRY(upload_extra(ctx, r, h.row, &d.row));
+    return upload_extra(ctx, r, h.val, &d.val);
+}
+static int32_t upload_density(bzk_ctx *ctx, bzk_r1cs *r, const std::vector<uint32_t> &a_idx, const std::vector<uint32_t> &b_idx) {
+    r->a_len = a_idx.size(); r->b_len = b_idx.size();
+    BZK_CUDA(ctx, cudaMalloc(&r->d_a_idx, (a_idx.size() + 1) * 4));
+    BZK_CUDA(ctx, cudaMalloc(&r->d_b_idx, (b_idx.size() + 1) * 4));
+    BZK_CUDA(ctx, cudaMemcpyAsync(r->d_a_idx, a_idx.data(), a_idx.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    BZK_CUDA(ctx, cudaMemcpyAsync(r->d_b_idx, b_idx.data(), b_idx.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    return BZK_OK;
+}
 static void free_r1cs(bzk_r1cs *r) {
     for (auto &m : r->m) { if (m.rowptr) cudaFree(m.rowptr); if (m.col) cudaFree(m.col); if (m.val) cudaFree(m.val); }
+    for (void *p : r->extra) cudaFree(p);
     if (r->d_a_idx) cudaFree(r->d_a_idx);
     if (r->d_b_idx) cudaFree(r->d_b_idx);
     delete r;
@@ -166,7 +254,10 @@ static int32_t witness_side(bzk_ctx *ctx, const bzk_r1cs *cs, const Stage &sg, c
         if (!ev[s]) continue;
         BZK_CUDA(ctx, cudaMemsetAsync(ev[s] + cs->ncons, 0, (m - cs->ncons) * sizeof(Fr), st));
         if (cs->ncons) {
-            k_csr_spmv<<<div_up(cs->ncons, 256), 256, 0, st>>>(cs->m[s].rowptr, cs->m[s].col, cs->m[s].val, cs->ncons, sg.z, ev[s]);
+            if (cs->blocked)
+                k_blocked_spmv<<<div_up(cs->ncons, 256), 256, 0, st>>>(cs->shape, cs->m[s].rowptr, cs->m[s].col, cs->m[s].val, cs->ncons, sg.z, ev[s]);
+            else
+                k_csr_spmv<<<div_up(cs->ncons, 256), 256, 0, st>>>(cs->m[s].rowptr, cs->m[s].col, cs->m[s].val, cs->ncons, sg.z, ev[s]);
             BZK_LAUNCHED(ctx);
         }
     }
@@ -367,22 +458,103 @@ int32_t bzk_r1cs_upload(bzk_ctx *ctx, uint64_t num_inputs, uint64_t num_aux, uin
     for (uint64_t k = 0; k < a_rp[ncons]; k++) if (nonzero(a_val[k])) a_d[a_col[k]] = 1;
     for (uint64_t k = 0; k < b_rp[ncons]; k++) if (nonzero(b_val[k])) b_d[b_col[k]] = 1;
     std::vector<uint32_t> a_idx, b_idx;
-    for (uint64_t v = 0; v < num_inputs; v++) a_idx.push_back((uint32_t)v);
-    for (uint64_t v = num_inputs; v < nv; v++) if (a_d[v]) a_idx.push_back((uint32_t)v);
-    for (uint64_t v = 0; v < nv; v++) if (b_d[v]) b_idx.push_back((uint32_t)v);
-    r->a_len = a_idx.size(); r->b_len = b_idx.size();
+    density_lists(num_inputs, a_d, b_d, a_idx, b_idx);
     int32_t st = BZK_OK;
     for (int s = 0; s < 3 && st == BZK_OK; s++) st = upload_csr(ctx, r->m[s], ncons, rp[s], cl[s], vl[s]);
+    if (st == BZK_OK) st = upload_density(ctx, r, a_idx, b_idx);
     if (st == BZK_OK) {
-        cudaError_t e = cudaMalloc(&r->d_a_idx, (a_idx.size() + 1) * 4);
-        if (e == cudaSuccess) e = cudaMalloc(&r->d_b_idx, (b_idx.size() + 1) * 4);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(r->d_a_idx, a_idx.data(), a_idx.size() * 4, cudaMemcpyHostToDevice, ctx->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(r->d_b_idx, b_idx.data(), b_idx.size() * 4, cudaMemcpyHostToDevice, ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+        cudaError_t e = cudaStreamSynchronize(ctx->stream);
         if (e != cudaSuccess) st = set_cuda_err(ctx, e, "r1cs upload", __FILE__, __LINE__);
     }
     if (st != BZK_OK) { free_r1cs(r); return st; }
     *out = r;
+    return BZK_OK;
+}
+
+/* include/bzk.h: the stored rows head | template | tail per side; validated on the host before anything is allocated */
+int32_t bzk_r1cs_upload_blocked(bzk_ctx *ctx, uint64_t num_inputs, uint64_t num_aux, uint64_t head_rows, uint64_t tmpl_rows, uint64_t reps,
+                                uint64_t tail_rows, uint64_t var_lo, uint64_t var_stride, const uint64_t *const rowptr[3], const uint32_t *const col[3],
+                                const bzk_fr *const val[3], bzk_r1cs **out) {
+    if (!ctx || !out || !rowptr || !col || !val || num_inputs == 0) return BZK_ERR_BAD_ARG;
+    *out = nullptr;
+    const uint64_t nv = num_inputs + num_aux;
+    if (nv < num_inputs || nv > (1ull << 32)) return BZK_ERR_BAD_ARG;
+    BlockedShape b;
+    b.head_rows = head_rows; b.tmpl_rows = tmpl_rows; b.reps = reps; b.tail_rows = tail_rows; b.var_lo = var_lo; b.var_stride = var_stride;
+    // the logical row count must not wrap (and stays far below 2^32: the domain is at most 2^28)
+    if (head_rows > (1ull << 32) || tmpl_rows > (1ull << 32) || tail_rows > (1ull << 32) || (tmpl_rows && reps > (1ull << 32) / tmpl_rows))
+        return BZK_ERR_BAD_ARG;
+    for (int s = 0; s < 3; s++)
+        if (!blocked_valid(b, nv, rowptr[s], col[s], val[s])) return BZK_ERR_BAD_ARG;
+    const uint64_t ncons = b.rows();
+    uint32_t log_m = 0;
+    while ((1ull << log_m) < ncons + num_inputs) log_m++;
+    if (log_m > 28) return BZK_ERR_BAD_ARG;
+    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+    bzk_r1cs *r = new (std::nothrow) bzk_r1cs();
+    if (!r) return BZK_ERR_OOM;
+    r->num_inputs = num_inputs; r->num_aux = num_aux; r->ncons = ncons; r->log_m = log_m;
+    r->blocked = true;
+    r->shape = b;
+    std::vector<uint8_t> a_d(nv, 0), b_d(nv, 0);
+    blocked_presence(b, rowptr[0], col[0], (const Fr *)val[0], a_d);
+    blocked_presence(b, rowptr[1], col[1], (const Fr *)val[1], b_d);
+    std::vector<uint32_t> a_idx, b_idx;
+    density_lists(num_inputs, a_d, b_d, a_idx, b_idx);
+    auto upload = [&]() -> int32_t {
+        for (int s = 0; s < 3; s++) {
+            BZK_TRY(upload_csr(ctx, r->m[s], b.stored_rows(), rowptr[s], col[s], val[s]));
+            const HostBlockedT h = blocked_transpose(b, rowptr[s], col[s], (const Fr *)val[s]);
+            DevBlockedT &d = r->t[s];
+            d.span = h.span;
+            BZK_TRY(upload_extra(ctx, r, h.s_ptr, &d.s_ptr));
+            BZK_TRY(upload_extra(ctx, r, h.s_row, &d.s_row));
+            BZK_TRY(upload_extra(ctx, r, h.s_val, &d.s_val));
+            BZK_TRY(upload_col_list(ctx, r, h.shared, d.shared));
+            BZK_TRY(upload_col_list(ctx, r, h.fixed, d.fixed));
+            BZK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the host vectors go out of scope
+        }
+        BZK_TRY(upload_density(ctx, r, a_idx, b_idx));
+        BZK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        return BZK_OK;
+    };
+    const int32_t st = upload();
+    if (st != BZK_OK) { free_r1cs(r); return st; }
+    *out = r;
+    return BZK_OK;
+}
+
+/* d_out[j] = sum_row M_side[row][j] * d_lag[row] for every variable j, on the context's stream (blocked handles) */
+int32_t bzk_r1cs_columns_dev(bzk_ctx *ctx, const bzk_r1cs *r, uint32_t side, const void *d_lag, void *d_out) {
+    if (!ctx || !r || !r->blocked || side > 2 || !d_lag || !d_out) return BZK_ERR_BAD_ARG;
+    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+    const BlockedShape &b = r->shape;
+    const DevBlockedT &t = r->t[side];
+    const Fr *lag = (const Fr *)d_lag;
+    Fr *o = (Fr *)d_out;
+    const uint64_t nv = r->num_inputs + r->num_aux;
+    cudaStream_t st = ctx->stream;
+    k_blocked_slot_cols<<<div_up(nv, 256), 256, 0, st>>>(b, t.span, t.s_ptr, t.s_row, t.s_val, lag, nv, o);
+    BZK_LAUNCHED(ctx);
+    if (t.shared.n) {
+        Fr *sums = nullptr;
+        BZK_CUDA(ctx, cudaMalloc(&sums, b.tmpl_rows * sizeof(Fr)));
+        k_blocked_rowsum<<<div_up(b.tmpl_rows, 256), 256, 0, st>>>(b, lag, sums);
+        cudaError_t e = cudaGetLastError();
+        if (e == cudaSuccess) {
+            ctx->launches++;
+            k_col_list_add<<<div_up(t.shared.n, 256), 256, 0, st>>>(t.shared.n, t.shared.col, t.shared.ptr, t.shared.row, t.shared.val, sums, o);
+            e = cudaGetLastError();
+            ctx->launches++;
+        }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        cudaFree(sums);
+        if (e != cudaSuccess) return set_cuda_err(ctx, e, "r1cs columns", __FILE__, __LINE__);
+    }
+    if (t.fixed.n) {
+        k_col_list_add<<<div_up(t.fixed.n, 256), 256, 0, st>>>(t.fixed.n, t.fixed.col, t.fixed.ptr, t.fixed.row, t.fixed.val, lag, o);
+        BZK_LAUNCHED(ctx);
+    }
     return BZK_OK;
 }
 
@@ -428,6 +600,50 @@ int32_t bzk_g2_fixed_base_mul_dev(bzk_ctx *ctx, const bzk_g2_affine *base, const
     if (n == 0) return BZK_OK;
     k_fixed_base_g2<<<div_up(n, 64), 64, 0, ctx->stream>>>(from_wire(base), (const Fr *)d_scalars, n, (uint8_t *)d_out);
     BZK_LAUNCHED(ctx);
+    return BZK_OK;
+}
+
+/* k_fixed_base_g1 / _g2 into a new resident vector: bases[i] = [k_i] base, never held as wire images */
+int32_t bzk_g1_bases_fixed_base_mul(bzk_ctx *ctx, const bzk_g1_affine *base, const void *d_scalars, size_t n, bzk_g1_bases **out) {
+    if (!ctx || !base || !out || (n && !d_scalars)) return BZK_ERR_BAD_ARG;
+    *out = nullptr;
+    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+    bzk_g1_bases *b = new (std::nothrow) bzk_g1_bases();
+    if (!b) return BZK_ERR_OOM;
+    b->n = n;
+    cudaError_t e = cudaMalloc(&b->d, (n ? n : 1) * sizeof(G1Affine));
+    if (e == cudaSuccess && n) {
+        k_fixed_base_packed_g1<<<div_up(n, 128), 128, 0, ctx->stream>>>(from_wire(base), (const Fr *)d_scalars, n, b->d);
+        ctx->launches++;
+        e = cudaGetLastError();
+    }
+    if (e != cudaSuccess) {
+        if (b->d) cudaFree(b->d);
+        delete b;
+        return set_cuda_err(ctx, e, "g1 fixed-base bases", __FILE__, __LINE__);
+    }
+    *out = b;
+    return BZK_OK;
+}
+int32_t bzk_g2_bases_fixed_base_mul(bzk_ctx *ctx, const bzk_g2_affine *base, const void *d_scalars, size_t n, bzk_g2_bases **out) {
+    if (!ctx || !base || !out || (n && !d_scalars)) return BZK_ERR_BAD_ARG;
+    *out = nullptr;
+    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+    bzk_g2_bases *b = new (std::nothrow) bzk_g2_bases();
+    if (!b) return BZK_ERR_OOM;
+    b->n = n;
+    cudaError_t e = cudaMalloc(&b->d, (n ? n : 1) * sizeof(G2Affine));
+    if (e == cudaSuccess && n) {
+        k_fixed_base_packed_g2<<<div_up(n, 64), 64, 0, ctx->stream>>>(from_wire(base), (const Fr *)d_scalars, n, b->d);
+        ctx->launches++;
+        e = cudaGetLastError();
+    }
+    if (e != cudaSuccess) {
+        if (b->d) cudaFree(b->d);
+        delete b;
+        return set_cuda_err(ctx, e, "g2 fixed-base bases", __FILE__, __LINE__);
+    }
+    *out = b;
     return BZK_OK;
 }
 

@@ -759,20 +759,24 @@ struct bzk_mpn_circuit {
     uint64_t reveal_vars = 0;
     std::vector<int32_t> row_local;  // where each entry of the revealed row sits in the phase-1 block
     std::vector<int32_t> ext_src;    // per phase-2 external: -1 = the entering state, else the phase-1 RAW index it copies
+    // update circuit: {head_rows, tmpl_rows, reps, tail_rows, var_lo, var_stride} (bzk_mpn_circuit_blocks); a blocked
+    // compile stores head | template | tail only, and nnz[] counts the entries of the expanded matrices
+    bool blocked = false;
+    uint64_t blocks[6] = {0, 0, 0, 0, 0, 0};
+    uint64_t nnz[3] = {0, 0, 0};
 };
 
-extern "C" {
-
-/* poseidon_blob: bazuka_b200/data/poseidon_params.bin (the table bzk_poseidon_load_params takes);
- * jubjub = {d, 8*BASE.x, 8*BASE.y} canonical */
-int32_t bzk_mpn_update_circuit_compile(uint32_t log4_tree, uint32_t log4_token, uint32_t log4_batch, const uint8_t *poseidon_blob, size_t blob_len,
-                                       const bzk_fr jubjub[3], bzk_mpn_circuit **out) {
+// The update circuit.  blocked: slots >= 2 advance the variable and row counts without storing their rows, so the
+// matrices hold head | template (slot 1) | tail, the form bzk_r1cs_upload_blocked takes.
+static int32_t update_circuit_compile(uint32_t log4_tree, uint32_t log4_token, uint32_t log4_batch, const uint8_t *poseidon_blob, size_t blob_len,
+                                      const bzk_fr jubjub[3], bool blocked, bzk_mpn_circuit **out) {
     if (!poseidon_blob || !jubjub || !out || blob_len < 12 || memcmp(poseidon_blob, "BZKPOSv1", 8) || log4_tree == 0 || log4_tree > 31 ||
         log4_token == 0 || log4_token > 8 || log4_batch > 6)
         return BZK_ERR_BAD_ARG;
     std::unique_ptr<bzk_mpn_circuit> c(new (std::nothrow) bzk_mpn_circuit);
     if (!c) return BZK_ERR_OOM;
     c->A = log4_tree; c->T = log4_token; c->B = log4_batch;
+    c->blocked = blocked;
     cc::Ctx cx;
     if (!cc::load_constants(poseidon_blob, blob_len, jubjub, &cx)) return BZK_ERR_BAD_ARG;
     const uint64_t n = 1ull << (2 * log4_batch);
@@ -809,7 +813,8 @@ int32_t bzk_mpn_update_circuit_compile(uint32_t log4_tree, uint32_t log4_token, 
             for (int s = 0; s < 3; s++) before[s] = cs.m[s].col.size();
             const uint64_t aux_before = cs.n_aux;
             o = cc::tx_block(cs, cx, log4_tree, log4_token, state, p.fee_token);
-            if (k == 0 && n > 1)  // every slot emits the same amount: size the arrays once instead of doubling through GBs
+            if (k == 0) rows_lo = rows_hi = cs.m[0].rowptr.size();  // the template is empty unless slot 1 exists
+            if (k == 0 && n > 1 && !blocked)  // every slot emits the same amount: size the arrays once instead of doubling through GBs
                 for (int s = 0; s < 3; s++) {
                     const size_t per = cs.m[s].col.size() - before[s], rows_per = cs.m[s].rowptr.size() - rows_before;
                     cs.m[s].col.reserve(cs.m[s].col.size() + per * (n - 1) + 4096);
@@ -824,7 +829,7 @@ int32_t bzk_mpn_update_circuit_compile(uint32_t log4_tree, uint32_t log4_token, 
             }
         } else {
             const uint64_t shift = 2 * (k - 1) * a_tx;  // Var encoding: aux j = 2j + 1
-            for (int s = 0; s < 3; s++) {
+            for (int s = 0; s < 3 && !blocked; s++) {
                 cc::Csr &m = cs.m[s];
                 const size_t base = m.col.size() - chunk_lo[s];
                 for (size_t i = chunk_lo[s]; i < chunk_hi[s]; i++) {
@@ -854,7 +859,12 @@ int32_t bzk_mpn_update_circuit_compile(uint32_t log4_tree, uint32_t log4_token, 
     }
     cs.recipes.clear();
     cs.recipes.shrink_to_fit();
+    // rowptr[r] for r in [rows_lo, rows_hi) ends slot 1's rows: the head is the rows before it
+    const uint64_t head = rows_lo - 1, tmpl = rows_hi - rows_lo, reps = n - 1;
+    const uint64_t blocks[6] = {head, tmpl, reps, cs.n_rows - head - tmpl * reps, cs.n_inputs + first_block, n > 1 ? a_tx : c->slot_vars};
+    memcpy(c->blocks, blocks, sizeof blocks);
     for (int s = 0; s < 3; s++) {
+        c->nnz[s] = cs.m[s].col.size() + (blocked && n > 2 ? (n - 2) * (chunk_hi[s] - chunk_lo[s]) : 0);
         c->col[s].resize(cs.m[s].col.size());
         for (size_t i = 0; i < cs.m[s].col.size(); i++) {
             const cc::Var v = cs.m[s].col[i];
@@ -867,6 +877,27 @@ int32_t bzk_mpn_update_circuit_compile(uint32_t log4_tree, uint32_t log4_token, 
     return BZK_OK;
 }
 
+extern "C" {
+
+/* poseidon_blob: bazuka_b200/data/poseidon_params.bin (the table bzk_poseidon_load_params takes);
+ * jubjub = {d, 8*BASE.x, 8*BASE.y} canonical */
+int32_t bzk_mpn_update_circuit_compile(uint32_t log4_tree, uint32_t log4_token, uint32_t log4_batch, const uint8_t *poseidon_blob, size_t blob_len,
+                                       const bzk_fr jubjub[3], bzk_mpn_circuit **out) {
+    return update_circuit_compile(log4_tree, log4_token, log4_batch, poseidon_blob, blob_len, jubjub, false, out);
+}
+int32_t bzk_mpn_update_circuit_compile_blocked(uint32_t log4_tree, uint32_t log4_token, uint32_t log4_batch, const uint8_t *poseidon_blob,
+                                               size_t blob_len, const bzk_fr jubjub[3], bzk_mpn_circuit **out) {
+    return update_circuit_compile(log4_tree, log4_token, log4_batch, poseidon_blob, blob_len, jubjub, true, out);
+}
+
+/* out[9] = {head_rows, tmpl_rows, reps, tail_rows, var_lo, var_stride, stored nnz a, b, c}; update circuits only */
+int32_t bzk_mpn_circuit_blocks(const bzk_mpn_circuit *c, uint64_t out[9]) {
+    if (!c || !out || c->kind != 0) return BZK_ERR_BAD_ARG;
+    memcpy(out, c->blocks, sizeof c->blocks);
+    for (int s = 0; s < 3; s++) out[6 + s] = c->col[s].size();
+    return BZK_OK;
+}
+
 int32_t bzk_mpn_circuit_free(bzk_mpn_circuit *c) {
     delete c;
     return BZK_OK;
@@ -876,7 +907,8 @@ int32_t bzk_mpn_circuit_free(bzk_mpn_circuit *c) {
  *              epilogue_vars, 0} */
 int32_t bzk_mpn_circuit_shape(const bzk_mpn_circuit *c, uint64_t shape[12]) {
     if (!c || !shape) return BZK_ERR_BAD_ARG;
-    const uint64_t s[12] = {c->cs.n_inputs, c->cs.n_aux, c->cs.n_rows, c->col[0].size(), c->col[1].size(), c->col[2].size(),
+    const uint64_t s[12] = {c->cs.n_inputs, c->cs.n_aux, c->cs.n_rows, c->kind ? c->col[0].size() : c->nnz[0], c->kind ? c->col[1].size() : c->nnz[1],
+                            c->kind ? c->col[2].size() : c->nnz[2],
                             c->p_aux, c->slot_vars, c->state_out, c->final_fee, c->epi.ops.size() / 6, c->reveal_vars};
     memcpy(shape, s, sizeof s);
     return BZK_OK;
@@ -889,7 +921,8 @@ int32_t bzk_mpn_circuit_kind(const bzk_mpn_circuit *c, uint32_t out[4]) {
     return BZK_OK;
 }
 
-/* side = 0,1,2 (A,B,C): rowptr u64[ncons+1], col u32[nnz], val Fr[nnz] (Montgomery) — the arrays of bzk_r1cs_upload */
+/* side = 0,1,2 (A,B,C): rowptr u64[ncons+1], col u32[nnz], val Fr[nnz] (Montgomery) — the arrays of bzk_r1cs_upload; of a
+ * blocked compile, the stored rows head | template | tail (sizes from bzk_mpn_circuit_blocks) */
 int32_t bzk_mpn_circuit_matrix(const bzk_mpn_circuit *c, uint32_t side, uint64_t *rowptr, uint32_t *col, bzk_fr *val) {
     if (!c || side > 2 || !rowptr || !col || !val) return BZK_ERR_BAD_ARG;
     memcpy(rowptr, c->cs.m[side].rowptr.data(), c->cs.m[side].rowptr.size() * 8);

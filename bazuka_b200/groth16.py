@@ -93,6 +93,91 @@ class R1CS:
         return trp, rows[order].astype(np.uint32), val[order]
 
 
+class BlockedR1CS:
+    """A constraint system whose middle is one block of rows repeated `reps` times, stored once (bzk_r1cs_upload_blocked).
+    Logical rows: head_rows explicit rows | reps copies of the tmpl_rows template rows | tail_rows explicit rows; each side's
+    CSR (rowptr, col, val as in R1CS) holds the stored rows head | template | tail.  A template column c >= var_lo names
+    c + k*var_stride in copy k; a smaller one names c in every copy.  An MPN update batch from
+    NativeUpdateCircuit(..., blocked=True).blocked_r1cs() is this with one slot as the template."""
+
+    def __init__(self, num_inputs, num_aux, head_rows, tmpl_rows, reps, tail_rows, var_lo, var_stride, a, b, c):
+        self.num_inputs, self.num_aux = int(num_inputs), int(num_aux)
+        self.head_rows, self.tmpl_rows, self.reps, self.tail_rows = int(head_rows), int(tmpl_rows), int(reps), int(tail_rows)
+        self.var_lo, self.var_stride = int(var_lo), int(var_stride)
+        stored = self.head_rows + self.tmpl_rows + self.tail_rows
+        self.mats = []
+        for rp, col, val in (a, b, c):
+            rp = np.ascontiguousarray(rp, dtype=np.uint64)
+            col = np.ascontiguousarray(col, dtype=np.uint32)
+            val = np.ascontiguousarray(val, dtype=np.uint64).reshape(-1, 4)
+            assert len(rp) == stored + 1 and rp[0] == 0 and rp[-1] == len(col) == len(val)
+            self.mats.append((rp, col, val))
+        self.num_constraints = self.head_rows + self.tmpl_rows * self.reps + self.tail_rows
+
+    num_vars = R1CS.num_vars
+    log_m = R1CS.log_m
+
+    @property
+    def blocks(self):
+        return self.head_rows, self.tmpl_rows, self.reps, self.tail_rows, self.var_lo, self.var_stride
+
+    def _parts(self, k):
+        """matrix k's stored rows as (head, template, tail), each (row lengths, col, val)"""
+        rp, col, val = self.mats[k]
+        cut = [0, self.head_rows, self.head_rows + self.tmpl_rows, len(rp) - 1]
+        return [(np.diff(rp[a:b + 1]), col[rp[a]:rp[b]], val[rp[a]:rp[b]]) for a, b in zip(cut, cut[1:])]
+
+    def expand(self):
+        """the explicit R1CS (numpy; for tests and small sizes: it materialises every copy)"""
+        mats = []
+        for k in range(3):
+            (hl, hc, hv), (tl, tc, tv), (xl, xc, xv) = self._parts(k)
+            slot = tc >= self.var_lo
+            shifts = np.arange(self.reps, dtype=np.uint64) * np.uint64(self.var_stride)
+            tcols = [np.where(slot, tc.astype(np.uint64) + sh, tc.astype(np.uint64)) for sh in shifts]
+            lens = np.concatenate([hl] + [tl] * self.reps + [xl]).astype(np.uint64)
+            rp = np.zeros(len(lens) + 1, dtype=np.uint64)
+            np.cumsum(lens, out=rp[1:])
+            col = np.concatenate([hc.astype(np.uint64)] + tcols + [xc.astype(np.uint64)]).astype(np.uint32)
+            val = np.concatenate([hv] + [tv] * self.reps + [xv]).reshape(-1, 4)
+            mats.append((rp, col, val))
+        return R1CS(self.num_inputs, self.num_aux, *mats)
+
+    def density(self):
+        """R1CS.density of the expansion, from the blocks (every copy of a template slot column is present)"""
+        pres = []
+        for k in range(2):
+            d = np.zeros(self.num_vars, dtype=bool)
+            (hl, hc, hv), (tl, tc, tv), (xl, xc, xv) = self._parts(k)
+            for c, v in ((hc, hv), (xc, xv)):
+                d[c[v.any(axis=1)]] = True
+            if self.reps:
+                tc = tc[tv.any(axis=1)]
+                d[tc[tc < self.var_lo]] = True
+                rel = np.unique(tc[tc >= self.var_lo]).astype(np.int64)
+                for k0 in range(0, self.reps, 64):
+                    ks = np.arange(k0, min(k0 + 64, self.reps), dtype=np.int64) * self.var_stride
+                    d[(rel[None, :] + ks[:, None]).reshape(-1)] = True
+            pres.append(d)
+        a_idx = np.concatenate([np.arange(self.num_inputs), self.num_inputs + np.nonzero(pres[0][self.num_inputs:])[0]])
+        b_idx = np.nonzero(pres[1])[0]
+        return a_idx.astype(np.uint32), b_idx.astype(np.uint32)
+
+
+def _upload_r1cs(ctx, r1cs):
+    """a bzk_r1cs handle for an R1CS (bzk_r1cs_upload) or a BlockedR1CS (bzk_r1cs_upload_blocked)"""
+    h = ct.c_void_p()
+    if isinstance(r1cs, BlockedR1CS):
+        arr = lambda i: (ct.c_void_p * 3)(*[m[i].ctypes.data for m in r1cs.mats])
+        ctx._check(ctx._l.bzk_r1cs_upload_blocked(ctx._h, r1cs.num_inputs, r1cs.num_aux, *r1cs.blocks, arr(0), arr(1), arr(2), ct.byref(h)))
+        return h
+    args = []
+    for rp, col, val in r1cs.mats:
+        args += [_host_ptr(rp), _host_ptr(col), _host_ptr(val)]
+    ctx._check(ctx._l.bzk_r1cs_upload(ctx._h, r1cs.num_inputs, r1cs.num_aux, r1cs.num_constraints, *args, ct.byref(h)))
+    return h
+
+
 class ProvingKey:
     def __init__(self, ctx, handle, vk):
         self._ctx, self._h, self.vk = ctx, handle, vk
@@ -209,16 +294,11 @@ def write_parameters(ctx, pk, dest=None):
 
 
 class Prover:
-    """One circuit on one GPU: the R1CS and (optionally) its proving key resident in HBM."""
+    """One circuit on one GPU: the R1CS (an R1CS or a BlockedR1CS) and (optionally) its proving key resident in HBM."""
 
-    def __init__(self, ctx: Context, r1cs: R1CS):
+    def __init__(self, ctx: Context, r1cs):
         self.ctx, self.r1cs = ctx, r1cs
-        h = ct.c_void_p()
-        args = []
-        for rp, col, val in r1cs.mats:
-            args += [_host_ptr(rp), _host_ptr(col), _host_ptr(val)]
-        ctx._check(ctx._l.bzk_r1cs_upload(ctx._h, r1cs.num_inputs, r1cs.num_aux, r1cs.num_constraints, *args, ct.byref(h)))
-        self._h = h
+        self._h = _upload_r1cs(ctx, r1cs)
         shp = np.zeros(5, dtype=np.uint64)
         ctx._check(ctx._l.bzk_r1cs_shape(self._h, _host_ptr(shp)))
         self.log_m, self.h_len, self.l_len, self.a_len, self.b_len = (int(x) for x in shp)
@@ -469,10 +549,13 @@ def zkproof_blob(proof_bytes):
 # ------------------------------------------------------------------------------------------------
 # trusted setup on the GPU (bellman `generate_parameters`, explicit toxic waste)
 # ------------------------------------------------------------------------------------------------
-def setup_gpu(ctx: Context, r1cs: R1CS, toxic, g1_image, g2_image, table_levels=None):
+def setup_gpu(ctx: Context, r1cs, toxic, g1_image, g2_image, table_levels=None):
     """toxic = [tau, alpha, beta, gamma, delta] as [5,4] Montgomery; g1/g2: generator wire images.
     Returns (ProvingKey, vk dict).  All field/group work runs in libbzk kernels; numpy only moves
-    and reorders data.  table_levels: as in proving_key_from_host."""
+    and reorders data.  table_levels: as in proving_key_from_host.
+    r1cs: an R1CS (the key keeps its wire images in pk.device_images), or a BlockedR1CS: the Lagrange columns come from
+    bzk_r1cs_columns_dev, each vector is multiplied straight into its resident form and every temporary is dropped before
+    the next vector is made, so the device never holds a vector twice; no wire images are kept.  Both give the same key."""
     import torch
     # torch slicing / indexing kernels and libbzk kernels interleave below: put both on one stream
     ctx.use_torch_stream()
@@ -531,6 +614,9 @@ def _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels):
     zd = s_mul(zt, dinv)
     h_k = mul(d_pw[: m - 1].contiguous(), rep(zd, m - 1))                  # tau^i Z(tau)/delta
     ctx.ntt_dev(d_pw, log_m, NTT_IFFT)                                     # d_pw <- L_j(tau)
+    if isinstance(r1cs, BlockedR1CS):
+        step = seg = None
+        return _setup_blocked(ctx, r1cs, toxic, g1_image, g2_image, table_levels, d_pw, h_k, dinv, ginv, dev, rep, mul, add)
     lag = d_pw
     cols = []
     for k in range(3):
@@ -584,6 +670,83 @@ def _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels):
     pk = _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels)
     pk.device_images = host  # wire images kept for tests / export
     return pk, vk
+
+
+def _setup_blocked(ctx, r1cs, toxic, g1_image, g2_image, table_levels, lag, h_k, dinv, ginv, dev, rep, mul, add):
+    """the rest of _setup_gpu for a BlockedR1CS (lag = L_j(tau), h_k = tau^i Z(tau)/delta): the same key, built one
+    resident vector at a time"""
+    import torch
+    t = torch
+    from .api import G1Bases, G2Bases
+    ni, na, nc, nv, m = r1cs.num_inputs, r1cs.num_aux, r1cs.num_constraints, r1cs.num_vars, 1 << r1cs.log_m
+    g1_image = np.ascontiguousarray(g1_image, dtype=np.uint8)
+    g2_image = np.ascontiguousarray(g2_image, dtype=np.uint8)
+
+    def bases(kind, scal):
+        out = ct.c_void_p()
+        n = scal.shape[0]
+        fn = ctx._l.bzk_g1_bases_fixed_base_mul if kind == 1 else ctx._l.bzk_g2_bases_fixed_base_mul
+        ctx._check(fn(ctx._h, _host_ptr(g1_image if kind == 1 else g2_image), _p(scal.contiguous()) if n else None, n, ct.byref(out)))
+        ctx.synchronize()
+        return (G1Bases if kind == 1 else G2Bases)(ctx, out)
+
+    def drop():
+        torch.cuda.synchronize()
+        torch.cuda.empty_cache()   # hand freed temporaries back before libbzk allocates the next vector
+
+    hb = bases(1, h_k)
+    del h_k
+    drop()
+    h = _upload_r1cs(ctx, r1cs)
+    try:
+        cols = []
+        for k in range(3):
+            out = t.empty((nv, 4), dtype=t.int64, device="cuda")
+            ctx._check(ctx._l.bzk_r1cs_columns_dev(ctx._h, h, k, _p(lag), _p(out)))
+            cols.append(out)
+        ctx.synchronize()
+    finally:
+        ctx._check(ctx._l.bzk_r1cs_free(ctx._h, h))
+    at, bt, ctv = cols
+    del cols
+    at[:ni] = add(at[:ni].contiguous(), lag[nc:nc + ni].contiguous())   # the Input(i) * 0 = 0 rows
+    del lag
+    ext = add(add(mul(at, rep(toxic[2], nv)), mul(bt, rep(toxic[1], nv))), ctv)
+    del ctv
+    ext_ic = mul(ext[:ni].contiguous(), rep(ginv, ni))
+    ext_l = mul(ext[ni:].contiguous(), rep(dinv, na)) if na else ext[ni:]
+    del ext
+    drop()
+    lb = bases(1, ext_l)
+    del ext_l
+    drop()
+    a_idx, b_idx = r1cs.density()
+    ab = bases(1, at[t.from_numpy(a_idx.astype(np.int64)).cuda()])
+    del at
+    drop()
+    bsc = bt[t.from_numpy(b_idx.astype(np.int64)).cuda()]
+    del bt
+    drop()
+    b1b = bases(1, bsc)
+    b2b = bases(2, bsc)
+    del bsc
+    drop()
+
+    def images(kind, scal):
+        n = scal.shape[0]
+        w = G1_BYTES if kind == 1 else G2_BYTES
+        out = t.empty((max(n, 1), w), dtype=t.uint8, device="cuda")
+        fn = ctx._l.bzk_g1_fixed_base_mul_dev if kind == 1 else ctx._l.bzk_g2_fixed_base_mul_dev
+        ctx._check(fn(ctx._h, _host_ptr(g1_image if kind == 1 else g2_image), _p(scal.contiguous()), n, _p(out)))
+        return out[:n].cpu().numpy()
+
+    tox = dev(toxic)
+    ic = images(1, ext_ic)
+    vk_g1 = images(1, tox[[1, 2, 4]])      # alpha, beta, delta
+    vk_g2 = images(2, tox[[2, 3, 4]])      # beta, gamma, delta
+    vk = {"alpha_g1": vk_g1[0], "beta_g1": vk_g1[1], "delta_g1": vk_g1[2],
+          "beta_g2": vk_g2[0], "gamma_g2": vk_g2[1], "delta_g2": vk_g2[2], "ic": ic}
+    return _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels), vk
 
 
 def _p(tensor):

@@ -3,6 +3,8 @@
     nc = NativeUpdateCircuit(A, T, B)           # no GPU needed
     ni, na, mats = nc.r1cs()                     # the arrays of groth16.R1CS / bzk_r1cs_upload
     slot, epi = nc.program(0), nc.program(1)     # witness_program.WitnessProgram objects
+    NativeUpdateCircuit(A, T, B, blocked=True).blocked_r1cs()
+                                                 # groth16.BlockedR1CS: one slot stored, the others are its copies
 
 The Python definition in this package (cs.py, gadgets.py, update.py) stays as the readable restatement and the
 test oracle for it: tests compare every emitted array."""
@@ -23,16 +25,21 @@ def _canon(v):
 
 
 class NativeUpdateCircuit:
-    def __init__(self, A, T, B):
+    """blocked=True: bzk_mpn_update_circuit_compile_blocked — slots 2.. are not stored (blocked_r1cs()); the shape and the
+    witness programs are those of the explicit compile"""
+    blocked = False
+
+    def __init__(self, A, T, B, blocked=False):
         from .. import _lib
         self._l = _lib.load()
-        self.A, self.T, self.B = A, T, B
+        self.A, self.T, self.B, self.blocked = A, T, B, blocked
         blob = open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "data", "poseidon_params.bin"), "rb").read()
         jj = np.ascontiguousarray(np.stack([_canon(N.JJ_D), _canon(N.JJ_BASE_COFACTOR[0]), _canon(N.JJ_BASE_COFACTOR[1])]))
         h = ct.c_void_p()
-        st = self._l.bzk_mpn_update_circuit_compile(A, T, B, blob, len(blob), ct.c_void_p(jj.ctypes.data), ct.byref(h))
+        name = "bzk_mpn_update_circuit_compile_blocked" if blocked else "bzk_mpn_update_circuit_compile"
+        st = getattr(self._l, name)(A, T, B, blob, len(blob), ct.c_void_p(jj.ctypes.data), ct.byref(h))
         if st != 0:
-            raise _lib.BzkError(st, "bzk_mpn_update_circuit_compile")
+            raise _lib.BzkError(st, name)
         self._h = h
         shape = np.zeros(12, dtype=np.uint64)
         self._l.bzk_mpn_circuit_shape(h, ct.c_void_p(shape.ctypes.data))
@@ -44,15 +51,39 @@ class NativeUpdateCircuit:
             self._l.bzk_mpn_circuit_free(self._h)
             self._h = None
 
-    def r1cs(self):
+    def blocks(self):
+        """bzk_mpn_circuit_blocks: (head_rows, tmpl_rows, reps, tail_rows, var_lo, var_stride), (stored nnz a, b, c)"""
+        out = np.zeros(9, dtype=np.uint64)
+        st = self._l.bzk_mpn_circuit_blocks(self._h, ct.c_void_p(out.ctypes.data))
+        if st != 0:
+            from .._lib import BzkError
+            raise BzkError(st, "bzk_mpn_circuit_blocks")
+        v = [int(x) for x in out]
+        return tuple(v[:6]), tuple(v[6:])
+
+    def _matrices(self, rows, nnzs):
         mats = []
-        for side, nnz in enumerate((self.nnz_a, self.nnz_b, self.nnz_c)):
-            rp = np.zeros(self.num_constraints + 1, dtype=np.uint64)
+        for side, nnz in enumerate(nnzs):
+            rp = np.zeros(rows + 1, dtype=np.uint64)
             col = np.zeros(max(nnz, 1), dtype=np.uint32)
             val = np.zeros((max(nnz, 1), 4), dtype=np.uint64)
             self._l.bzk_mpn_circuit_matrix(self._h, side, ct.c_void_p(rp.ctypes.data), ct.c_void_p(col.ctypes.data), ct.c_void_p(val.ctypes.data))
             mats.append((rp, col[:nnz], val[:nnz]))
-        return self.num_inputs, self.num_aux, mats
+        return mats
+
+    def r1cs(self):
+        if self.blocked:
+            e = self.blocked_r1cs().expand()
+            return e.num_inputs, e.num_aux, e.mats
+        return self.num_inputs, self.num_aux, self._matrices(self.num_constraints, (self.nnz_a, self.nnz_b, self.nnz_c))
+
+    def blocked_r1cs(self):
+        """groth16.BlockedR1CS of a blocked compile (of an explicit one it would hold every slot: use r1cs())"""
+        from ..groth16 import BlockedR1CS
+        assert self.blocked
+        blocks, nnzs = self.blocks()
+        head, tmpl, _, tail = blocks[:4]
+        return BlockedR1CS(self.num_inputs, self.num_aux, *blocks, *self._matrices(head + tmpl + tail, nnzs))
 
     def program(self, which) -> WitnessProgram:
         sizes = np.zeros(6, dtype=np.uint64)

@@ -215,6 +215,23 @@ int32_t bzk_r1cs_upload(bzk_ctx *ctx, uint64_t num_inputs, uint64_t num_aux, uin
 int32_t bzk_r1cs_free(bzk_ctx *ctx, bzk_r1cs *r1cs);
 /* out = { log2 m, |h| = m-1, |l|, |a|, |b_g1| = |b_g2| } the parameter vectors must have */
 int32_t bzk_r1cs_shape(const bzk_r1cs *r1cs, uint64_t out[5]);
+/* A blocked R1CS: a circuit whose middle is one block of rows repeated `reps` times, held once.  Logical rows, in order:
+ * head_rows explicit rows, reps copies of the tmpl_rows template rows, tail_rows explicit rows; each side's CSR
+ * (rowptr[head_rows + tmpl_rows + tail_rows + 1], col, val) stores head | template | tail.  Head and tail columns are z
+ * indices.  A template column c >= var_lo names c + k * var_stride in copy k (0-based); a template column c < var_lo
+ * names c in every copy.  An MPN update batch is head = prologue + slot 0, template = slot 1, reps = n - 1, var_lo =
+ * num_inputs + the prologue's aux count, var_stride = one slot's variables, tail = epilogue (bzk_mpn_circuit_blocks).
+ * The handle is an ordinary bzk_r1cs for bzk_r1cs_shape / _free and every prover entry point, with the density lists
+ * bzk_r1cs_upload would derive from the expanded matrices.  BZK_ERR_BAD_ARG, before anything is allocated: a rowptr
+ * that does not start at 0 or decreases, a missing array, an expanded column (the last copy's included) >= num_inputs +
+ * num_aux, num_inputs + num_aux > 2^32, or var_stride = 0 with reps > 0. */
+int32_t bzk_r1cs_upload_blocked(bzk_ctx *ctx, uint64_t num_inputs, uint64_t num_aux, uint64_t head_rows, uint64_t tmpl_rows, uint64_t reps,
+                                uint64_t tail_rows, uint64_t var_lo, uint64_t var_stride, const uint64_t *const rowptr[3], const uint32_t *const col[3],
+                                const bzk_fr *const val[3], bzk_r1cs **out);
+/* The transposed product the trusted setup needs: d_out[j] = sum_row M_side[row][j] * d_lag[row] for every variable j
+ * (side 0, 1, 2 = A, B, C; d_lag has one entry per logical row, d_out num_inputs + num_aux), on the context's stream,
+ * without atomics.  Blocked handles only: BZK_ERR_BAD_ARG for an explicit one. */
+int32_t bzk_r1cs_columns_dev(bzk_ctx *ctx, const bzk_r1cs *r1cs, uint32_t side, const void *d_lag, void *d_out);
 /* adopts the five resident base vectors (freed with the handle) plus the vk points the tail needs */
 int32_t bzk_groth16_params_create(bzk_ctx *ctx, const bzk_g1_affine *alpha_g1, const bzk_g1_affine *beta_g1, const bzk_g2_affine *beta_g2,
                                   const bzk_g1_affine *delta_g1, const bzk_g2_affine *delta_g2,
@@ -418,6 +435,14 @@ int32_t bzk_mpn_circuit_kind(const bzk_mpn_circuit *circuit, uint32_t out[4]);
  *          final_fee (slot-local), epilogue_vars, reveal_vars (two-phase circuits; 0 for the update circuit)} */
 int32_t bzk_mpn_circuit_shape(const bzk_mpn_circuit *circuit, uint64_t shape[12]);
 int32_t bzk_mpn_circuit_matrix(const bzk_mpn_circuit *circuit, uint32_t side, uint64_t *rowptr, uint32_t *col, bzk_fr *val);
+/* The update circuit in the blocked form of bzk_r1cs_upload_blocked: slots 2.. are not stored, so the matrices
+ * (bzk_mpn_circuit_matrix) hold head | template | tail.  The witness programs and bzk_mpn_circuit_shape (the expanded
+ * system's constraint and entry counts) equal bzk_mpn_update_circuit_compile's. */
+int32_t bzk_mpn_update_circuit_compile_blocked(uint32_t log4_tree, uint32_t log4_token, uint32_t log4_batch, const uint8_t *poseidon_blob,
+                                               size_t blob_len, const bzk_fr jubjub[3], bzk_mpn_circuit **out);
+/* out = {head_rows, tmpl_rows, reps, tail_rows, var_lo, var_stride, stored nnz a, b, c} of an update circuit from either
+ * compile (of an explicit one: where the blocks lie in its full matrices); BZK_ERR_BAD_ARG for the two-phase circuits */
+int32_t bzk_mpn_circuit_blocks(const bzk_mpn_circuit *circuit, uint64_t out[9]);
 /* which: 0 = slot program (two-phase circuits: phase 1), 1 = epilogue program (phase 2), 2 = the `reveal` of a two-phase
  * batch (one instance; externals = every slot's revealed row, slot-major); sizes = {n_ops, n_lc, n_terms, n_coefs, n_raw,
  * n_ext}; array outputs optional */
@@ -582,6 +607,10 @@ int32_t bzk_groth16_verify_batch_dev(bzk_ctx *ctx, const bzk_groth16_pvk *pvk, c
 int32_t bzk_csr_spmv_dev(bzk_ctx *ctx, const void *d_rowptr, const void *d_col, const void *d_val, uint64_t nrows, const void *d_vec, void *d_out);
 int32_t bzk_g1_fixed_base_mul_dev(bzk_ctx *ctx, const bzk_g1_affine *base, const void *d_scalars, size_t n, void *d_out);
 int32_t bzk_g2_fixed_base_mul_dev(bzk_ctx *ctx, const bzk_g2_affine *base, const void *d_scalars, size_t n, void *d_out);
+/* The same multiplications stored straight into a new resident base vector (d_scalars: n Montgomery Fr on the device),
+ * so that a key vector is never held twice; enqueued on the context's stream. */
+int32_t bzk_g1_bases_fixed_base_mul(bzk_ctx *ctx, const bzk_g1_affine *base, const void *d_scalars, size_t n, bzk_g1_bases **out);
+int32_t bzk_g2_bases_fixed_base_mul(bzk_ctx *ctx, const bzk_g2_affine *base, const void *d_scalars, size_t n, bzk_g2_bases **out);
 
 /* ------------------------------------------------------------------ elementwise Fr (device)
  * out[i] = a[i] (op) b[i]; used by the prover pipeline and the arithmetic parity tests. */
