@@ -22,14 +22,16 @@ int32_t tree4_versioned_update(bzk_ctx *ctx, uint32_t depth, const uint32_t *d_t
 int32_t groth16_h_launch(bzk_ctx *ctx, Fr *a, Fr *b, Fr *c, uint32_t log_n);
 int32_t groth16_h_combine_launch(bzk_ctx *ctx, Fr *a, Fr *b, Fr *c, uint32_t log_n);
 
-__global__ void __launch_bounds__(256) k_fr_binop(int op, const Fr *__restrict__ a, const Fr *__restrict__ b, Fr *__restrict__ out, size_t n) {
+// out may be a or b (in-place calls): the pointers are not __restrict__, and each element is read, through the
+// read-only path, only by the thread that then writes it, so no thread reads a location after it has been written
+__global__ void __launch_bounds__(256) k_fr_binop(int op, const Fr *a, const Fr *b, Fr *out, size_t n) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     Fr x = load_vec(a + i), y = load_vec(b + i);
     Fr r = op == BZK_FR_ADD ? x + y : (op == BZK_FR_SUB ? x - y : x * y);
     store_vec(out + i, r);
 }
-__global__ void __launch_bounds__(256) k_fp_mul(const Fp *__restrict__ a, const Fp *__restrict__ b, Fp *__restrict__ out, size_t n) {
+__global__ void __launch_bounds__(256) k_fp_mul(const Fp *a, const Fp *b, Fp *out, size_t n) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     store_vec(out + i, load_vec(a + i) * load_vec(b + i));

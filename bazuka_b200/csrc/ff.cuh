@@ -155,15 +155,17 @@ struct Fe {
         for (int i = 0; i < N; i++) r.l[i] = borrow ? a.l[i] : t.l[i];
         return r;
     }
+    // BZK_HOST_DEVICE_TEXT (tests only) makes a host build run the device text everywhere, so that sqr, inv, pow and the
+    // group law are checked on the CPU through add_limbs32 / sub_limbs32 / mul_evenodd as well
     BZK_HD friend Fe operator+(const Fe &a, const Fe &b) {
-#if defined(__CUDA_ARCH__)
+#if defined(__CUDA_ARCH__) || defined(BZK_HOST_DEVICE_TEXT)
         return add_limbs32(a, b);
 #else
         return add_host64(a, b);
 #endif
     }
     BZK_HD friend Fe operator-(const Fe &a, const Fe &b) {
-#if defined(__CUDA_ARCH__)
+#if defined(__CUDA_ARCH__) || defined(BZK_HOST_DEVICE_TEXT)
         return sub_limbs32(a, b);
 #else
         return sub_host64(a, b);
@@ -262,7 +264,7 @@ struct Fe {
     BZK_HD friend Fe operator*(const Fe &a, const Fe &b) {
 #if defined(__CUDA_ARCH__) && defined(BZK_MUL_NOINLINE)
         return mul_call(a, b);   // one out-of-line copy per translation unit: code-size experiment (instruction cache)
-#elif defined(__CUDA_ARCH__)
+#elif defined(__CUDA_ARCH__) || defined(BZK_HOST_DEVICE_TEXT)
         return mul_evenodd(a, b);
 #else
         return mul_host64(a, b);
@@ -555,7 +557,7 @@ struct Fe {
 
 // ---------------------------------------------------------------------------------------------
 // BLS12-381 parameter packs.  Limbs as constexpr switch tables so that they fold to immediates.
-// (R, R^2, inv are checked against big-integer arithmetic in tests/test_host_arith.py.)
+// (p, R, R^2 and inv are checked against big-integer arithmetic in tests/test_arith_edges_cpu.py.)
 // ---------------------------------------------------------------------------------------------
 #define BZK_TABLE(name, ...)                                   \
     BZK_HD static constexpr uint32_t name(int i) {             \
