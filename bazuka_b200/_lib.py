@@ -42,6 +42,8 @@ SIGNATURES = {
     "bzk_ctx_set_msm_affine_rounds": (_i32, [_vp, _i32, _i32]),
     "bzk_ctx_set_msm_table_window": (_i32, [_vp, _u32]),
     "bzk_ctx_last_msm_plan": (_i32, [_vp, _vp]),
+    "bzk_ctx_set_msm_stream_chunk": (_i32, [_vp, _u64]),
+    "bzk_ctx_last_msm_stream": (_i32, [_vp, _vp]),
     "bzk_ctx_stage_ms": (_u64, [_vp, _vp, _vp, _u32]),
     "bzk_poseidon_load_params": (_i32, [_vp, _vp, _sz]),
     "bzk_poseidon_hash": (_i32, [_vp, _u32, _vp, _sz, _vp]),
@@ -67,6 +69,10 @@ SIGNATURES = {
     "bzk_g2_bases_free": (_i32, [_vp, _vp]),
     "bzk_g1_bases_len": (_sz, [_vp]),
     "bzk_g2_bases_len": (_sz, [_vp]),
+    "bzk_g1_bases_move": (_i32, [_vp, _vp, _i32]),
+    "bzk_g2_bases_move": (_i32, [_vp, _vp, _i32]),
+    "bzk_g1_bases_on_host": (_i32, [_vp]),
+    "bzk_g2_bases_on_host": (_i32, [_vp]),
     "bzk_msm_g1_resident": (_i32, [_vp, _vp, _sz, _vp, _sz, _vp]),
     "bzk_msm_g2_resident": (_i32, [_vp, _vp, _sz, _vp, _sz, _vp]),
     "bzk_msm_g1_resident_dev": (_i32, [_vp, _vp, _sz, _vp, _sz, _vp]),
@@ -89,6 +95,8 @@ SIGNATURES = {
     "bzk_groth16_params_precompute": (_i32, [_vp, _vp, ct.c_uint32, ct.c_uint32]),
     "bzk_groth16_params_file_info": (_i32, [_vp, _sz, _vp]),
     "bzk_groth16_params_read": (_i32, [_vp, _vp, _sz, _i32] + [_vp] * 7 + [_sz, ct.POINTER(_vp)]),
+    "bzk_groth16_params_read_placed": (_i32, [_vp, _vp, _sz, _i32] + [_vp] * 7 + [_sz, _u32, ct.POINTER(_vp)]),
+    "bzk_groth16_params_move": (_i32, [_vp, _vp, _u32]),
     "bzk_groth16_params_write": (_i32, [_vp, _vp, _vp, _vp, _sz, _vp, _sz, ct.POINTER(_sz)]),
     "bzk_g1_bases_precompute": (_i32, [_vp, _vp, ct.c_uint32]),
     "bzk_g2_bases_precompute": (_i32, [_vp, _vp, ct.c_uint32]),

@@ -67,6 +67,21 @@ class _Bases:
     def levels(self):
         return int(getattr(self._ctx._l, f"bzk_{self._kind}_bases_levels")(self._h))
 
+    def move_to_host(self):
+        """put the points in pinned host memory and free their device storage, tables included (bzk_g*_bases_move): a
+        vector need not fit in device memory; its MSMs stream it to the device in chunks, with the same results."""
+        self._ctx._check(getattr(self._ctx._l, f"bzk_{self._kind}_bases_move")(self._ctx._h, self._h, 1))
+        return self
+
+    def move_to_device(self):
+        """back to device memory, untabled"""
+        self._ctx._check(getattr(self._ctx._l, f"bzk_{self._kind}_bases_move")(self._ctx._h, self._h, 0))
+        return self
+
+    @property
+    def on_host(self):
+        return bool(getattr(self._ctx._l, f"bzk_{self._kind}_bases_on_host")(self._h))
+
     def __del__(self):
         try:
             self.free()
@@ -75,7 +90,7 @@ class _Bases:
 
 
 class G1Bases(_Bases):
-    """Device-resident packed G1 base vector (one `Parameters<Bls12>` column)."""
+    """Packed G1 base vector (one `Parameters<Bls12>` column), on the device or in pinned host memory."""
     _kind = "g1"
 
 
@@ -142,6 +157,20 @@ class Context:
     def set_msm_table_window(self, c=0):
         """window of the fixed-base tables built from now on (8..23); 0 = the planner's choice.  Results unchanged."""
         self._check(self._l.bzk_ctx_set_msm_table_window(self._h, int(c)))
+
+    def set_msm_stream_chunk(self, points=0):
+        """points per device chunk buffer of the sums over host-resident vectors (>= 256); 0 = the library default.
+        Results unchanged."""
+        self._check(self._l.bzk_ctx_set_msm_stream_chunk(self._h, int(points)))
+
+    MSM_STREAM_FIELDS = ("chunks", "chunk_points", "bytes_h2d", "streamed")
+
+    def last_msm_stream(self):
+        """how the last single MSM on this context used its bases (bzk_ctx_last_msm_stream) as a dict of
+        MSM_STREAM_FIELDS; all 0 for a device vector."""
+        out = np.zeros(4, dtype=np.uint64)
+        self._check(self._l.bzk_ctx_last_msm_stream(self._h, _host_ptr(out)))
+        return dict(zip(self.MSM_STREAM_FIELDS, (int(x) for x in out)))
 
     MSM_PLAN_FIELDS = ("c", "W", "T", "G", "NB", "slice", "nbits", "long_len")
 

@@ -79,6 +79,42 @@ static int32_t bases_from_dev(bzk_ctx *ctx, const void *d_images, size_t n, int3
     return BZK_OK;
 }
 
+// every stream of the context that may still read a base vector: its own, the side streams and the pipes' copy streams
+static int32_t sync_all_streams(bzk_ctx *ctx) {
+    BZK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (cudaStream_t st : ctx->aux_stream)
+        if (st) BZK_CUDA(ctx, cudaStreamSynchronize(st));
+    for (const StreamPipe &p : ctx->pipe)
+        if (p.copy) BZK_CUDA(ctx, cudaStreamSynchronize(p.copy));
+    return BZK_OK;
+}
+
+// level 0 of the vector into new storage on the other side, then the old storage is freed (so a vector never exists
+// twice on the device); tables are dropped.  On failure the vector stays where it was.
+template <class B>
+static int32_t bases_move(bzk_ctx *ctx, B *b, bool to_host) {
+    if ((b->h != nullptr) == to_host) return BZK_OK;
+    BZK_TRY(sync_all_streams(ctx));
+    B moved;
+    moved.n = b->n;
+    BZK_TRY(bases_alloc(ctx, &moved, to_host));
+    void *dst = to_host ? (void *)moved.h : (void *)moved.d;
+    const void *src = to_host ? (const void *)b->d : (const void *)b->h;
+    cudaError_t e = cudaMemcpyAsync(dst, src, b->n * sizeof(*b->d), to_host ? cudaMemcpyDeviceToHost : cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) {
+        if (moved.h) cudaFreeHost(moved.h);
+        if (moved.d) cudaFree(moved.d);
+        return set_cuda_err(ctx, e, "base vector move", __FILE__, __LINE__);
+    }
+    if (b->d) cudaFree(b->d);
+    if (b->h) cudaFreeHost(b->h);
+    b->d = moved.d;
+    b->h = moved.h;
+    b->tab_c = 0; b->tab_T = 1; b->tab_G = 0;
+    return BZK_OK;
+}
+
 template <class B, class A, class IMG>
 static int32_t bases_upload(bzk_ctx *ctx, const IMG *host, size_t n, int32_t check, B **out,
                             int32_t (*pack)(bzk_ctx *, const uint8_t *, size_t, A *, uint32_t *)) {
@@ -144,6 +180,14 @@ int32_t bzk_ctx_destroy(bzk_ctx *ctx) {
     if (ctx->stage) cudaFree(ctx->stage);
     if (ctx->pinned) cudaFreeHost(ctx->pinned);
     for (auto &w : ctx->aux_ws) if (w) cudaFree(w);
+    for (auto &p : ctx->pipe) {
+        if (p.copy) { cudaStreamSynchronize(p.copy); cudaStreamDestroy(p.copy); }
+        if (p.buf) cudaFree(p.buf);
+        for (int b = 0; b < 2; b++) {
+            if (p.ready[b]) cudaEventDestroy(p.ready[b]);
+            if (p.freed[b]) cudaEventDestroy(p.freed[b]);
+        }
+    }
     for (auto &st : ctx->aux_stream) if (st) cudaStreamDestroy(st);
     for (auto &e : ctx->aux_ev) if (e) cudaEventDestroy(e);
     for (auto &e : ctx->ev) if (e) cudaEventDestroy(e);
@@ -178,6 +222,16 @@ int32_t bzk_ctx_set_msm_affine_rounds(bzk_ctx *ctx, int32_t g1_rounds, int32_t g
 int32_t bzk_ctx_set_msm_table_window(bzk_ctx *ctx, uint32_t c) {
     if (!ctx || (c != 0 && (c < 8 || c > 23))) return BZK_ERR_BAD_ARG;
     ctx->table_c = c;
+    return BZK_OK;
+}
+int32_t bzk_ctx_set_msm_stream_chunk(bzk_ctx *ctx, uint64_t points) {
+    if (!ctx || (points != 0 && points < 256) || points >= (1ull << 31)) return BZK_ERR_BAD_ARG;
+    ctx->stream_chunk = points;
+    return BZK_OK;
+}
+int32_t bzk_ctx_last_msm_stream(const bzk_ctx *ctx, uint64_t out[4]) {
+    if (!ctx || !out) return BZK_ERR_BAD_ARG;
+    memcpy(out, ctx->last_stream, sizeof ctx->last_stream);
     return BZK_OK;
 }
 int32_t bzk_ctx_last_msm_plan(const bzk_ctx *ctx, uint32_t out[8]) {
@@ -331,28 +385,38 @@ int32_t bzk_g1_bases_free(bzk_ctx *ctx, bzk_g1_bases *b) {
     BZK_ENTER(ctx);
     if (!b) return BZK_OK;
     BZK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (b->d) cudaFree(b->d);
-    delete b;
+    bases_release(b);
     return BZK_OK;
 }
 int32_t bzk_g2_bases_free(bzk_ctx *ctx, bzk_g2_bases *b) {
     BZK_ENTER(ctx);
     if (!b) return BZK_OK;
     BZK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (b->d) cudaFree(b->d);
-    delete b;
+    bases_release(b);
     return BZK_OK;
 }
 int32_t bzk_g1_bases_precompute(bzk_ctx *ctx, bzk_g1_bases *b, uint32_t max_levels) {
     BZK_ENTER(ctx);
-    if (!b) return BZK_ERR_BAD_ARG;
+    if (!b || b->h) return BZK_ERR_BAD_ARG;
     return precompute_g1(ctx, b, max_levels);
 }
 int32_t bzk_g2_bases_precompute(bzk_ctx *ctx, bzk_g2_bases *b, uint32_t max_levels) {
     BZK_ENTER(ctx);
-    if (!b) return BZK_ERR_BAD_ARG;
+    if (!b || b->h) return BZK_ERR_BAD_ARG;
     return precompute_g2(ctx, b, max_levels);
 }
+int32_t bzk_g1_bases_move(bzk_ctx *ctx, bzk_g1_bases *b, int32_t to_host) {
+    BZK_ENTER(ctx);
+    if (!b) return BZK_ERR_BAD_ARG;
+    return bases_move(ctx, b, to_host != 0);
+}
+int32_t bzk_g2_bases_move(bzk_ctx *ctx, bzk_g2_bases *b, int32_t to_host) {
+    BZK_ENTER(ctx);
+    if (!b) return BZK_ERR_BAD_ARG;
+    return bases_move(ctx, b, to_host != 0);
+}
+int32_t bzk_g1_bases_on_host(const bzk_g1_bases *b) { return b && b->h ? 1 : 0; }
+int32_t bzk_g2_bases_on_host(const bzk_g2_bases *b) { return b && b->h ? 1 : 0; }
 uint32_t bzk_g1_bases_levels(const bzk_g1_bases *b) { return b ? b->tab_T : 0; }
 uint32_t bzk_g2_bases_levels(const bzk_g2_bases *b) { return b ? b->tab_T : 0; }
 size_t bzk_g1_bases_len(const bzk_g1_bases *b) { return b ? b->n : 0; }

@@ -30,6 +30,15 @@ struct MsmPlan {
 };
 constexpr uint32_t kMaxWinPoints = 320;  // >= G * (1 + nbits) for every plan make_plan can produce
 
+// What one sum needs to stream a host-resident base vector (msm_impl.cuh): a copy stream and two device chunk buffers,
+// grown only.  ready[b]: the copy into buffer b is done; freed[b]: the last kernel that read buffer b is done.
+struct StreamPipe {
+    cudaStream_t copy = nullptr;
+    void *buf = nullptr;
+    size_t bytes = 0;
+    cudaEvent_t ready[2] = {nullptr, nullptr}, freed[2] = {nullptr, nullptr};
+};
+
 struct NttTables {
     Fr *d_fwd = nullptr;  // omega^j, j < n/2
     Fr *d_inv = nullptr;  // omega^-j
@@ -65,6 +74,10 @@ struct bzk_ctx {
     void *aux_ws[4] = {nullptr, nullptr, nullptr, nullptr};
     size_t aux_ws_bytes[4] = {0, 0, 0, 0};
     cudaEvent_t aux_ev[3] = {nullptr, nullptr, nullptr};
+    // streamed sums over host vectors: pipe 0 serves the context's stream (single MSMs, the h sum), 1..4 the side streams
+    bzk::StreamPipe pipe[5];
+    uint64_t stream_chunk = 0;     // points per chunk buffer (0: the default of msm_impl.cuh), bzk_ctx_set_msm_stream_chunk
+    uint64_t last_stream[4] = {0};  // of the last single MSM: chunks, chunk points, bytes copied host->device, 1 if streamed
     // optional per-stage device timing (CUDA events on the launching stream), see bzk_ctx_set_timing
     bool timing = false;
     static constexpr int kMaxStages = 16;
@@ -82,15 +95,19 @@ struct bzk_ctx {
     bool split_open = false;        // a shard_begin is waiting for its shard_finish
 };
 
-// A resident base vector.  After bzk_g*_bases_precompute `d` holds tab_T levels of n points each: level t =
-// [2^(tab_c * tab_G * t)] P_i (level 0 = the bases), so that the windows t*G+g of every scalar share bucket group g.
+// A base vector, in one of two places.  On the device, `d` holds it; after bzk_g*_bases_precompute `d` holds tab_T levels
+// of n points each: level t = [2^(tab_c * tab_G * t)] P_i (level 0 = the bases), so that the windows t*G+g of every scalar
+// share bucket group g.  In host memory (bzk_g*_bases_move), `h` holds level 0 in pinned memory, `d` is null and there is
+// no table; its MSMs stream the points to the device.
 struct bzk_g1_bases {
     bzk::G1Affine *d = nullptr;
+    bzk::G1Affine *h = nullptr;
     size_t n = 0;
     uint32_t tab_c = 0, tab_T = 1, tab_G = 0;
 };
 struct bzk_g2_bases {
     bzk::G2Affine *d = nullptr;
+    bzk::G2Affine *h = nullptr;
     size_t n = 0;
     uint32_t tab_c = 0, tab_T = 1, tab_G = 0;
 };
@@ -113,12 +130,33 @@ struct BasesRef {
     const Affine<F> *tab = nullptr;
     size_t n_tab = 0, off = 0;
     uint32_t c = 0, T = 1, G = 0;  // c == 0: no table, the plan is free to choose its window
+    bool host = false;             // tab is pinned host memory: the sum streams it (msm_impl.cuh)
 };
 template <class B>
 inline auto bases_ref(const B *b, size_t off = 0) {
     BasesRef<decltype(b->d->x)> r;
-    r.tab = b->d; r.n_tab = b->n; r.off = off; r.c = b->tab_c; r.T = b->tab_T; r.G = b->tab_G;
+    r.tab = b->h ? b->h : b->d; r.n_tab = b->n; r.off = off; r.c = b->tab_c; r.T = b->tab_T; r.G = b->tab_G;
+    r.host = b->h != nullptr;
     return r;
+}
+// storage for a new n-point vector, in pinned host memory or on the device; BZK_ERR_OOM (size in the context's error)
+// when it cannot be had — a host vector never falls back to pageable memory
+template <class B>
+inline int32_t bases_alloc(bzk_ctx *ctx, B *b, bool on_host) {
+    const size_t bytes = (b->n ? b->n : 1) * sizeof(*b->d);
+    const cudaError_t e = on_host ? cudaHostAlloc((void **)&b->h, bytes, cudaHostAllocDefault) : cudaMalloc((void **)&b->d, bytes);
+    if (e == cudaSuccess) return BZK_OK;
+    cudaGetLastError();
+    if (on_host) b->h = nullptr; else b->d = nullptr;
+    snprintf(ctx->err, sizeof ctx->err, "%s(%zu bytes) for a base vector: %s", on_host ? "cudaHostAlloc" : "cudaMalloc", bytes, cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? BZK_ERR_OOM : BZK_ERR_CUDA;
+}
+// frees the vector's storage and the handle
+template <class B>
+inline void bases_release(B *b) {
+    if (b->d) cudaFree(b->d);
+    if (b->h) cudaFreeHost(b->h);
+    delete b;
 }
 }  // namespace bzk
 

@@ -24,8 +24,10 @@ int32_t precompute_g1(bzk_ctx *ctx, bzk_g1_bases *b, uint32_t max_levels);
 int32_t precompute_g2(bzk_ctx *ctx, bzk_g2_bases *b, uint32_t max_levels);
 int32_t groth16_h_launch(bzk_ctx *ctx, Fr *a, Fr *b, Fr *c, uint32_t log_n);
 int32_t groth16_to_coset_launch(bzk_ctx *ctx, Fr *v, uint32_t log_n);
-int32_t msm_g1_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, const BasesRef<Fp> &d_bases, const Fr *d_scalars, size_t n, void *h_win, MsmPlan *plan);
-int32_t msm_g2_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, const BasesRef<Fp2> &d_bases, const Fr *d_scalars, size_t n, void *h_win, MsmPlan *plan);
+int32_t msm_g1_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, StreamPipe *pipe, const BasesRef<Fp> &d_bases, const Fr *d_scalars,
+                       size_t n, void *h_win, MsmPlan *plan);
+int32_t msm_g2_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, StreamPipe *pipe, const BasesRef<Fp2> &d_bases, const Fr *d_scalars,
+                       size_t n, void *h_win, MsmPlan *plan);
 void msm_g1_finish(const MsmPlan *plan, const void *h_win, bzk_g1_affine *out);
 void msm_g2_finish(const MsmPlan *plan, const void *h_win, bzk_g2_affine *out);
 
@@ -282,7 +284,9 @@ constexpr size_t kWinBytes = kMaxWinPoints * sizeof(G2Xyzz);
 // The five sums are independent once z is on the device (h additionally needs the quotient): the gathers and the l, a,
 // b_g1, b_g2 sums run on side streams with their own arenas, behind what the main stream has enqueued so far, while the
 // main stream goes on to the quotient and the h sum.  So the latency-bound phases of one MSM (bucket reduction, side-list
-// folding) overlap the throughput-bound phases of the others.
+// folding) overlap the throughput-bound phases of the others.  A sum over a host-resident vector streams it through its own
+// pipe (ctx->pipe[k + 1]); its first chunks are copied at once, not behind aux_ev[0], since the bases do not depend on the
+// witness.
 static int32_t witness_sums(bzk_ctx *ctx, const bzk_groth16_params *pk, const bzk_r1cs *cs, const Stage &sg, const Slices &sl) {
     for (int k = 0; k < 4; k++)
         if (!ctx->aux_stream[k]) BZK_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->aux_stream[k], cudaStreamNonBlocking));
@@ -303,25 +307,25 @@ static int32_t witness_sums(bzk_ctx *ctx, const bzk_groth16_params *pk, const bz
     BZK_CUDA(ctx, cudaStreamWaitEvent(s_l, ctx->aux_ev[0], 0));
     BZK_CUDA(ctx, cudaStreamWaitEvent(s_a, ctx->aux_ev[0], 0));
     BZK_CUDA(ctx, cudaStreamWaitEvent(s_b1, ctx->aux_ev[0], 0));
-    BZK_TRY(msm_g1_enqueue(ctx, s_l, &ctx->aux_ws[0], &ctx->aux_ws_bytes[0], bases_ref(pk->l), sg.z + ni + sl.l_lo, sl.l_n, hw + 1 * kWinBytes, &plan[1]));
+    BZK_TRY(msm_g1_enqueue(ctx, s_l, &ctx->aux_ws[0], &ctx->aux_ws_bytes[0], &ctx->pipe[1], bases_ref(pk->l), sg.z + ni + sl.l_lo, sl.l_n, hw + 1 * kWinBytes, &plan[1]));
     k_gather_fr<<<div_up(cs->a_len, 256), 256, 0, s_a>>>(sg.z, cs->d_a_idx, cs->a_len, sg.gs_a);
     BZK_LAUNCHED(ctx);
-    BZK_TRY(msm_g1_enqueue(ctx, s_a, &ctx->aux_ws[1], &ctx->aux_ws_bytes[1], bases_ref(pk->a), sg.gs_a + sl.a_lo, sl.a_n, hw + 2 * kWinBytes, &plan[2]));
+    BZK_TRY(msm_g1_enqueue(ctx, s_a, &ctx->aux_ws[1], &ctx->aux_ws_bytes[1], &ctx->pipe[2], bases_ref(pk->a), sg.gs_a + sl.a_lo, sl.a_n, hw + 2 * kWinBytes, &plan[2]));
     if (cs->b_len) {
         k_gather_fr<<<div_up(cs->b_len, 256), 256, 0, s_b1>>>(sg.z, cs->d_b_idx, cs->b_len, sg.gs_b);
         BZK_LAUNCHED(ctx);
     }
     BZK_CUDA(ctx, cudaEventRecord(ctx->aux_ev[1], s_b1));
     BZK_CUDA(ctx, cudaStreamWaitEvent(s_b2, ctx->aux_ev[1], 0));
-    BZK_TRY(msm_g1_enqueue(ctx, s_b1, &ctx->aux_ws[2], &ctx->aux_ws_bytes[2], bases_ref(pk->b1), sg.gs_b + sl.b_lo, sl.b_n, hw + 3 * kWinBytes, &plan[3]));
-    BZK_TRY(msm_g2_enqueue(ctx, s_b2, &ctx->aux_ws[3], &ctx->aux_ws_bytes[3], bases_ref(pk->b2), sg.gs_b + sl.b_lo, sl.b_n, hw + 4 * kWinBytes, &plan[4]));
+    BZK_TRY(msm_g1_enqueue(ctx, s_b1, &ctx->aux_ws[2], &ctx->aux_ws_bytes[2], &ctx->pipe[3], bases_ref(pk->b1), sg.gs_b + sl.b_lo, sl.b_n, hw + 3 * kWinBytes, &plan[3]));
+    BZK_TRY(msm_g2_enqueue(ctx, s_b2, &ctx->aux_ws[3], &ctx->aux_ws_bytes[3], &ctx->pipe[4], bases_ref(pk->b2), sg.gs_b + sl.b_lo, sl.b_n, hw + 4 * kWinBytes, &plan[4]));
     for (int k = 0; k < 4; k++) g16_mark(ctx, 4 + k, ctx->aux_stream[k]);
     return BZK_OK;
 }
 
 // the h sum over n quotient coefficients at src, on the main stream
 static int32_t h_sum(bzk_ctx *ctx, const bzk_groth16_params *pk, const Fr *src, uint64_t n) {
-    BZK_TRY(msm_g1_enqueue(ctx, ctx->stream, &ctx->ws, &ctx->ws_bytes, bases_ref(pk->h), src, n, ctx->pinned, &ctx->g16_plan[0]));
+    BZK_TRY(msm_g1_enqueue(ctx, ctx->stream, &ctx->ws, &ctx->ws_bytes, &ctx->pipe[0], bases_ref(pk->h), src, n, ctx->pinned, &ctx->g16_plan[0]));
     g16_mark(ctx, 3, ctx->stream);
     return BZK_OK;
 }
@@ -696,24 +700,37 @@ int32_t bzk_groth16_stage_ms(const bzk_ctx *ctx, float out[8]) {
 /* Fixed-base tables for the five base vectors of a key (they never change between proofs): up to `max_levels` levels
  * [2^(c*G*t)] P per base, so that the windows of a scalar share ceil(W/levels) bucket groups — fewer, larger windows and
  * one bucket reduction per group instead of per window.  max_levels = 0 picks the largest count (<= 16) whose tables fit
- * in `mem_fraction_percent` % of the currently free device memory.  Memory: levels x the key's size. */
+ * in `mem_fraction_percent` % of the currently free device memory.  Memory: levels x the device vectors' size.  Vectors in
+ * host memory stay as they are: they have no tables. */
 int32_t bzk_groth16_params_precompute(bzk_ctx *ctx, bzk_groth16_params *p, uint32_t max_levels, uint32_t mem_fraction_percent) {
     if (!ctx || !p) return BZK_ERR_BAD_ARG;
     BZK_CUDA(ctx, cudaSetDevice(ctx->device));
     if (max_levels == 0) {
         size_t free_b = 0, total_b = 0;
         BZK_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
-        const double key_bytes = (double)(p->h->n + p->l->n + p->a->n + p->b1->n) * sizeof(G1Affine) + (double)p->b2->n * sizeof(G2Affine);
+        auto dev_n = [](const auto *b) { return b->h ? 0.0 : (double)b->n; };
+        const double key_bytes = (dev_n(p->h) + dev_n(p->l) + dev_n(p->a) + dev_n(p->b1)) * sizeof(G1Affine) + dev_n(p->b2) * sizeof(G2Affine);
         const double budget = (double)free_b * (mem_fraction_percent ? mem_fraction_percent : 50) / 100.0;
         uint32_t lv = key_bytes > 0 ? (uint32_t)(budget / key_bytes) + 1 : 16;  // level 0 is already resident
         max_levels = lv > 16 ? 16 : lv;
     }
     if (max_levels <= 1) return BZK_OK;
-    BZK_TRY(precompute_g1(ctx, p->h, max_levels));
-    BZK_TRY(precompute_g1(ctx, p->l, max_levels));
-    BZK_TRY(precompute_g1(ctx, p->a, max_levels));
-    BZK_TRY(precompute_g1(ctx, p->b1, max_levels));
-    BZK_TRY(precompute_g2(ctx, p->b2, max_levels));
+    for (bzk_g1_bases *b : {p->h, p->l, p->a, p->b1})
+        if (!b->h) BZK_TRY(precompute_g1(ctx, b, max_levels));
+    if (!p->b2->h) BZK_TRY(precompute_g2(ctx, p->b2, max_levels));
+    return BZK_OK;
+}
+
+/* the key's five vectors to pinned host memory (bit v of host_mask, order h, l, a, b_g1, b_g2) or to the device (bit
+ * clear); the moves to the host go first, so that device memory peaks no higher than before the call */
+int32_t bzk_groth16_params_move(bzk_ctx *ctx, bzk_groth16_params *p, uint32_t host_mask) {
+    if (!ctx || !p || host_mask > 31) return BZK_ERR_BAD_ARG;
+    bzk_g1_bases *g1[4] = {p->h, p->l, p->a, p->b1};
+    for (int to_host = 1; to_host >= 0; to_host--) {
+        for (int v = 0; v < 4; v++)
+            if ((int)((host_mask >> v) & 1) == to_host) BZK_TRY(bzk_g1_bases_move(ctx, g1[v], to_host));
+        if ((int)((host_mask >> 4) & 1) == to_host) BZK_TRY(bzk_g2_bases_move(ctx, p->b2, to_host));
+    }
     return BZK_OK;
 }
 

@@ -7,9 +7,9 @@ namespace bzk {
 int32_t msm_g1_run(bzk_ctx *ctx, const BasesRef<Fp> &d_bases, const Fr *d_scalars, size_t n, bzk_g1_affine *out) {
     return msm_run<Fp>(ctx, d_bases, d_scalars, n, out);
 }
-int32_t msm_g1_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, const BasesRef<Fp> &d_bases, const Fr *d_scalars, size_t n,
-                       void *h_win, MsmPlan *plan) {
-    return msm_enqueue<Fp>(ctx, st, ws, ws_bytes, false, d_bases, d_scalars, n, (Xyzz<Fp> *)h_win, plan);
+int32_t msm_g1_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, StreamPipe *pipe, const BasesRef<Fp> &d_bases,
+                       const Fr *d_scalars, size_t n, void *h_win, MsmPlan *plan) {
+    return msm_enqueue<Fp>(ctx, st, ws, ws_bytes, pipe, false, d_bases, d_scalars, n, (Xyzz<Fp> *)h_win, plan);
 }
 void msm_g1_finish(const MsmPlan *plan, const void *h_win, bzk_g1_affine *out) { msm_host_finish<Fp>(*plan, (const Xyzz<Fp> *)h_win, out); }
 int32_t precompute_g1(bzk_ctx *ctx, bzk_g1_bases *b, uint32_t max_levels) {

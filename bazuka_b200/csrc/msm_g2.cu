@@ -7,9 +7,9 @@ namespace bzk {
 int32_t msm_g2_run(bzk_ctx *ctx, const BasesRef<Fp2> &d_bases, const Fr *d_scalars, size_t n, bzk_g2_affine *out) {
     return msm_run<Fp2>(ctx, d_bases, d_scalars, n, out);
 }
-int32_t msm_g2_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, const BasesRef<Fp2> &d_bases, const Fr *d_scalars, size_t n,
-                       void *h_win, MsmPlan *plan) {
-    return msm_enqueue<Fp2>(ctx, st, ws, ws_bytes, false, d_bases, d_scalars, n, (Xyzz<Fp2> *)h_win, plan);
+int32_t msm_g2_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, StreamPipe *pipe, const BasesRef<Fp2> &d_bases,
+                       const Fr *d_scalars, size_t n, void *h_win, MsmPlan *plan) {
+    return msm_enqueue<Fp2>(ctx, st, ws, ws_bytes, pipe, false, d_bases, d_scalars, n, (Xyzz<Fp2> *)h_win, plan);
 }
 void msm_g2_finish(const MsmPlan *plan, const void *h_win, bzk_g2_affine *out) { msm_host_finish<Fp2>(*plan, (const Xyzz<Fp2> *)h_win, out); }
 int32_t precompute_g2(bzk_ctx *ctx, bzk_g2_bases *b, uint32_t max_levels) {

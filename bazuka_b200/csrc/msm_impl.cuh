@@ -30,6 +30,7 @@
 #pragma once
 #include "common.cuh"
 #include "msm_affine.cuh"
+#include <algorithm>
 #include <cstdlib>
 #ifndef BZK_ACC_MIN_BLOCKS_G1
 #define BZK_ACC_MIN_BLOCKS_G1 4
@@ -376,6 +377,19 @@ __global__ void __launch_bounds__(256) k_fixup_long(const Xyzz<F> *__restrict__ 
     }
 }
 
+// the chunks after the first of a streamed sum accumulate into a cleared pass array (so k_accumulate / k_fixup run
+// unchanged); this adds each bucket the chunk touched into the sum's buckets.  One thread per bucket, no atomics.
+template <class F>
+__global__ void __launch_bounds__(128) k_bucket_fold(Xyzz<F> *__restrict__ buckets, const Xyzz<F> *__restrict__ pass, uint32_t TB) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= TB) return;
+    const Xyzz<F> v = load_vec(pass + b);
+    if (v.is_inf()) return;
+    Xyzz<F> t = load_vec(buckets + b);
+    t.add(v);
+    store_vec(buckets + b, t);
+}
+
 // ---------------------------------------------------------------------------------------------
 // 6. bucket reduction: per window  sum_b (b+1) * B_b
 // ---------------------------------------------------------------------------------------------
@@ -557,22 +571,68 @@ static int32_t bases_precompute(bzk_ctx *ctx, Affine<F> **d, size_t n, uint32_t 
 // ---------------------------------------------------------------------------------------------
 // host driver
 // ---------------------------------------------------------------------------------------------
+// Points per chunk buffer of a streamed sum unless bzk_ctx_set_msm_stream_chunk says otherwise: 384 MB per buffer for G1 and
+// for G2, two buffers per sum.  A chunk is long enough that its digit / scan / reduction overheads stay small next to its
+// accumulation, and its copy (~8 ms at 50 GB/s) hides behind the accumulation of the one before.
+template <class F>
+static size_t stream_chunk_points(const bzk_ctx *ctx) {
+    if (ctx->stream_chunk) return (size_t)ctx->stream_chunk;
+    return sizeof(F) == sizeof(Fp) ? ((size_t)1 << 22) : ((size_t)1 << 21);
+}
+
+// the copy stream, events and at least `bytes` of chunk buffers of one pipe (grown only)
+static int32_t ensure_pipe(bzk_ctx *ctx, StreamPipe *p, cudaStream_t st, size_t bytes) {
+    if (!p->copy) BZK_CUDA(ctx, cudaStreamCreateWithFlags(&p->copy, cudaStreamNonBlocking));
+    for (int b = 0; b < 2; b++) {
+        if (!p->ready[b]) BZK_CUDA(ctx, cudaEventCreateWithFlags(&p->ready[b], cudaEventDisableTiming));
+        if (!p->freed[b]) BZK_CUDA(ctx, cudaEventCreateWithFlags(&p->freed[b], cudaEventDisableTiming));
+    }
+    if (p->bytes >= bytes) return BZK_OK;
+    if (p->buf) {
+        // the buffers' last users: copies on the pipe's stream, kernels on the sum's stream
+        BZK_CUDA(ctx, cudaStreamSynchronize(p->copy));
+        BZK_CUDA(ctx, cudaStreamSynchronize(st));
+        BZK_CUDA(ctx, cudaFree(p->buf));
+        p->buf = nullptr;
+        p->bytes = 0;
+    }
+    BZK_CUDA(ctx, cudaMalloc(&p->buf, bytes));
+    p->bytes = bytes;
+    return BZK_OK;
+}
+
 template <class F>
 // Enqueue one MSM on stream `st` with its own workspace arena; the W window sums are copied into
 // `h_win` (host, ideally pinned; >= 64 entries) by the last operation on the stream.  Nothing here
 // synchronises: several MSMs can be in flight on different streams (the Groth16 driver runs its
 // five sums concurrently), and msm_host_finish folds the window sums once the stream is done.
 // `d_long_len` (optional) receives the device address of the long-run queue length k_fixup counts.
-static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, bool timed, const BasesRef<F> &bases,
-                           const Fr *d_scalars, size_t n, Xyzz<F> *h_win, MsmPlan *plan_out, uint32_t **d_long_len = nullptr) {
+//
+// A host-resident vector (bases.host) is streamed through `pipe`: the sum runs in passes over chunks of its terms.  Each
+// chunk's points are copied on the pipe's stream into one of two device buffers while the previous chunk is accumulated;
+// the chunk's digits, scan and scatter index into that buffer.  The first chunk's accumulate / fixup fill the bucket array;
+// each later chunk's fill a cleared pass array that k_bucket_fold then adds into it.  One bucket reduction ends the sum,
+// as for a resident vector.  The first copies wait for nothing on `st`, so they overlap whatever `st` runs before the sum.
+// Streamed sums use no batched-affine rounds and record no stage marks.  `stream_out` (optional): chunks, chunk points,
+// bytes copied host->device, 1 if streamed.
+static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_bytes, StreamPipe *pipe, bool timed, const BasesRef<F> &bases,
+                           const Fr *d_scalars, size_t n, Xyzz<F> *h_win, MsmPlan *plan_out, uint32_t **d_long_len = nullptr,
+                           uint64_t *stream_out = nullptr) {
+    if (stream_out) memset(stream_out, 0, 4 * sizeof(uint64_t));
     if (n == 0) { plan_out->W = 0; return BZK_OK; }
     if (n >= ((size_t)1 << 31) || bases.off + n > bases.n_tab) return BZK_ERR_BAD_ARG;
+    const bool streamed = bases.host;
+    if (streamed && (bases.T != 1 || !pipe)) return BZK_ERR_BAD_ARG;
     const MsmPlan pl = make_plan(n, bases.c, bases.T, bases.G);
     if ((double)bases.n_tab * pl.T >= 2147483648.0) return BZK_ERR_BAD_ARG;
     const Affine<F> *d_bases = bases.tab;
     *plan_out = pl;
     if ((double)n * pl.W >= 4294967295.0) return BZK_ERR_BAD_ARG;
-    const uint64_t max_entries = (uint64_t)n * pl.W;
+    // terms per pass: all of them, or one chunk of a streamed sum
+    size_t cn = n;
+    if (streamed) cn = std::min(n, stream_chunk_points<F>(ctx));
+    const size_t passes = (n + cn - 1) / cn;
+    const uint64_t max_entries = (uint64_t)cn * pl.W;
 
     // thread geometry of the accumulate kernel
     const uint32_t acc_threads_target = (uint32_t)ctx->sm_count * 128 * (sizeof(F) == sizeof(Fp) ? BZK_ACC_MIN_BLOCKS_G1 : 2);
@@ -591,7 +651,7 @@ static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_
     const int ctx_rounds = ctx->affine_rounds[sizeof(F) == sizeof(Fp) ? 0 : 1];
     const int env_rounds = ctx_rounds >= 0 ? ctx_rounds : (sizeof(F) == sizeof(Fp) ? env_g1 : env_g2);
     uint32_t R = 0;
-    if (env_rounds > 0 && (double)bases.n_tab * pl.T < 1073741824.0 && max_entries >= 8ull * pl.TB) {
+    if (!streamed && env_rounds > 0 && (double)bases.n_tab * pl.T < 1073741824.0 && max_entries >= 8ull * pl.TB) {
         R = (uint32_t)env_rounds;
         while (R && (max_entries >> R) < 2ull * pl.TB) R--;   // stop when buckets are down to a couple of entries
     }
@@ -646,6 +706,7 @@ static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_
             cv.take<F>(rnd_blocks); cv.take<F>(rnd_blocks); cv.take<F>(rnd_blocks); cv.take<F>(4);
         }
         cv.take<Xyzz<F>>(pl.TB);
+        cv.take<Xyzz<F>>(passes > 1 ? pl.TB : 0);
         cv.take<Xyzz<F>>(nslots); cv.take<int32_t>(nslots);
         cv.take<LongRun>(kLongQueueCap); cv.take<uint32_t>(4);
         cv.take<Xyzz<F>>(nslices); cv.take<Xyzz<F>>(nslices);
@@ -672,6 +733,7 @@ static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_
         blk_tot = cv.take<F>(rnd_blocks); blk_pre = cv.take<F>(rnd_blocks); blk_suf = cv.take<F>(rnd_blocks); inv_total = cv.take<F>(4);
     }
     Xyzz<F> *buckets = cv.take<Xyzz<F>>(pl.TB);
+    Xyzz<F> *pass_buckets = cv.take<Xyzz<F>>(passes > 1 ? pl.TB : 0);  // a streamed sum's later chunks (k_bucket_fold)
     Xyzz<F> *part_pts = cv.take<Xyzz<F>>(nslots);
     int32_t *part_bucket = cv.take<int32_t>(nslots);
     LongRun *long_queue = cv.take<LongRun>(kLongQueueCap);
@@ -681,65 +743,95 @@ static int32_t msm_enqueue(bzk_ctx *ctx, cudaStream_t st, void **ws, size_t *ws_
     Xyzz<F> *partial = cv.take<Xyzz<F>>((size_t)rows * parts);
     Xyzz<F> *win_out = cv.take<Xyzz<F>>(rows);
 
+    Affine<F> *chunk_buf[2] = {nullptr, nullptr};
+    if (streamed) {
+        const size_t half = (cn * sizeof(Affine<F>) + 255) & ~(size_t)255;
+        BZK_TRY(ensure_pipe(ctx, pipe, st, 2 * half));
+        chunk_buf[0] = (Affine<F> *)pipe->buf;
+        chunk_buf[1] = (Affine<F> *)((char *)pipe->buf + half);
+        if (stream_out) {
+            stream_out[0] = passes; stream_out[1] = cn; stream_out[2] = (uint64_t)n * sizeof(Affine<F>); stream_out[3] = 1;
+        }
+    }
+
     // stage marks: 0 clear+digits/histogram, 1 scan, 2 scatter, 3 accumulate, 4 fixup,
     //              5 bucket slices, 6 window sums (+ D2H of W points)
     const bool saved_timing = ctx->timing;
-    ctx->timing = saved_timing && timed;
+    ctx->timing = saved_timing && timed && !streamed;
     timing_begin(ctx);
-    BZK_CUDA(ctx, cudaMemsetAsync(counts, 0, (pl.TB + 1) * sizeof(uint32_t), st));
     BZK_CUDA(ctx, cudaMemsetAsync(buckets, 0, (size_t)pl.TB * sizeof(Xyzz<F>), st));  // all-zero = identity
-
-    k_digits<false><<<div_up(n, 256), 256, 0, st>>>(d_scalars, n, pl.c, pl.W, pl.NB, pl.G, (uint32_t)bases.n_tab, (uint32_t)bases.off, counts, nullptr);
-    BZK_LAUNCHED(ctx);
-    timing_mark(ctx);
-    k_scan_tile_sums<<<ntiles, kScanBlock, 0, st>>>(counts, pl.TB, tile_sums);
-    BZK_LAUNCHED(ctx);
-    k_scan_tiles<<<1, 1024, 0, st>>>(tile_sums, ntiles);
-    BZK_LAUNCHED(ctx);
-    k_scan_apply<<<ntiles, kScanBlock, 0, st>>>(counts, pl.TB, tile_sums, ntiles, offsets, cursor);
-    BZK_LAUNCHED(ctx);
-    timing_mark(ctx);
-    k_digits<true><<<div_up(n, 256), 256, 0, st>>>(d_scalars, n, pl.c, pl.W, pl.NB, pl.G, (uint32_t)bases.n_tab, (uint32_t)bases.off, cursor, sorted);
-    BZK_LAUNCHED(ctx);
-    timing_mark(ctx);
-    const uint32_t *acc_list = sorted, *acc_off = offsets;
-    if (R) {
-        const size_t fsm = 2 * kRoundThreads * sizeof(F), msm_ = 2 * (size_t)mid_threads * sizeof(F);
-        BZK_CUDA(ctx, cudaFuncSetAttribute(k_round_mid<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm_));
-        uint32_t scr_base = 0;
-        for (uint32_t r = 0; r < R; r++) {
-            uint32_t *off1 = roff[r & 1], *list1 = rlist[r & 1];
-            k_round_counts<<<div_up(pl.TB + 1, 256), 256, 0, st>>>(acc_off, pl.TB, counts);
-            BZK_LAUNCHED(ctx);
-            k_scan_tile_sums<<<ntiles, kScanBlock, 0, st>>>(counts, pl.TB, tile_sums);
-            BZK_LAUNCHED(ctx);
-            k_scan_tiles<<<1, 1024, 0, st>>>(tile_sums, ntiles);
-            BZK_LAUNCHED(ctx);
-            k_scan_apply<<<ntiles, kScanBlock, 0, st>>>(counts, pl.TB, tile_sums, ntiles, off1, cursor);
-            BZK_LAUNCHED(ctx);
-            k_round_fwd<F><<<rnd_blocks, kRoundThreads, fsm, st>>>(d_bases, scr, acc_list, acc_off, off1, pl.TB, rpre, thr_pre, thr_suf, blk_tot);
-            BZK_LAUNCHED(ctx);
-            k_round_mid<F><<<1, mid_threads, msm_, st>>>(blk_tot, rnd_blocks, blk_pre, blk_suf, inv_total);
-            BZK_LAUNCHED(ctx);
-            k_round_bwd<F><<<rnd_blocks, kRoundThreads, 0, st>>>(d_bases, scr, scr_base, acc_list, acc_off, off1, pl.TB, rpre, thr_pre, thr_suf, blk_pre,
-                                                                 blk_suf, inv_total, list1);
-            BZK_LAUNCHED(ctx);
-            scr_base += (uint32_t)cap[r + 1];
-            acc_list = list1;
-            acc_off = off1;
+    const size_t fsmem = 256 * sizeof(Xyzz<F>);
+    BZK_CUDA(ctx, cudaFuncSetAttribute(k_fixup_long<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+    for (size_t pass = 0; pass < passes; pass++) {
+        const size_t p0 = pass * cn, pn = std::min(cn, n - p0);
+        const Fr *p_scalars = d_scalars + p0;
+        // a streamed chunk's entries index its buffer (offset 0); T == 1, so n_tab only has to match the launch's bound checks
+        const uint32_t p_tab = streamed ? (uint32_t)pn : (uint32_t)bases.n_tab, p_off = streamed ? 0u : (uint32_t)bases.off;
+        const int cb = (int)(pass & 1);
+        if (streamed) {
+            d_bases = chunk_buf[cb];
+            BZK_CUDA(ctx, cudaStreamWaitEvent(pipe->copy, pipe->freed[cb], 0));
+            BZK_CUDA(ctx, cudaMemcpyAsync(chunk_buf[cb], bases.tab + bases.off + p0, pn * sizeof(Affine<F>), cudaMemcpyHostToDevice, pipe->copy));
+            BZK_CUDA(ctx, cudaEventRecord(pipe->ready[cb], pipe->copy));
         }
-    }
-    k_accumulate<F><<<acc_blocks, 128, 0, st>>>(d_bases, R ? scr : nullptr, acc_list, acc_off, pl.TB, 16u, buckets, part_pts, part_bucket);
-    BZK_LAUNCHED(ctx);
-    timing_mark(ctx);
-    BZK_CUDA(ctx, cudaMemsetAsync(long_len, 0, 16, st));
-    k_fixup<F><<<div_up(nslots, 128), 128, 0, st>>>(part_pts, part_bucket, nslots, acc_off, pl.TB, acc_blocks * 128, 16u, buckets, long_queue, long_len);
-    BZK_LAUNCHED(ctx);
-    {
-        const size_t fsmem = 256 * sizeof(Xyzz<F>);
-        BZK_CUDA(ctx, cudaFuncSetAttribute(k_fixup_long<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-        k_fixup_long<F><<<ctx->sm_count, 256, fsmem, st>>>(part_pts, part_bucket, buckets, long_queue, long_len);
+        BZK_CUDA(ctx, cudaMemsetAsync(counts, 0, (pl.TB + 1) * sizeof(uint32_t), st));
+        k_digits<false><<<div_up(pn, 256), 256, 0, st>>>(p_scalars, pn, pl.c, pl.W, pl.NB, pl.G, p_tab, p_off, counts, nullptr);
         BZK_LAUNCHED(ctx);
+        timing_mark(ctx);
+        k_scan_tile_sums<<<ntiles, kScanBlock, 0, st>>>(counts, pl.TB, tile_sums);
+        BZK_LAUNCHED(ctx);
+        k_scan_tiles<<<1, 1024, 0, st>>>(tile_sums, ntiles);
+        BZK_LAUNCHED(ctx);
+        k_scan_apply<<<ntiles, kScanBlock, 0, st>>>(counts, pl.TB, tile_sums, ntiles, offsets, cursor);
+        BZK_LAUNCHED(ctx);
+        timing_mark(ctx);
+        k_digits<true><<<div_up(pn, 256), 256, 0, st>>>(p_scalars, pn, pl.c, pl.W, pl.NB, pl.G, p_tab, p_off, cursor, sorted);
+        BZK_LAUNCHED(ctx);
+        timing_mark(ctx);
+        const uint32_t *acc_list = sorted, *acc_off = offsets;
+        if (R) {
+            const size_t fsm = 2 * kRoundThreads * sizeof(F), msm_ = 2 * (size_t)mid_threads * sizeof(F);
+            BZK_CUDA(ctx, cudaFuncSetAttribute(k_round_mid<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)msm_));
+            uint32_t scr_base = 0;
+            for (uint32_t r = 0; r < R; r++) {
+                uint32_t *off1 = roff[r & 1], *list1 = rlist[r & 1];
+                k_round_counts<<<div_up(pl.TB + 1, 256), 256, 0, st>>>(acc_off, pl.TB, counts);
+                BZK_LAUNCHED(ctx);
+                k_scan_tile_sums<<<ntiles, kScanBlock, 0, st>>>(counts, pl.TB, tile_sums);
+                BZK_LAUNCHED(ctx);
+                k_scan_tiles<<<1, 1024, 0, st>>>(tile_sums, ntiles);
+                BZK_LAUNCHED(ctx);
+                k_scan_apply<<<ntiles, kScanBlock, 0, st>>>(counts, pl.TB, tile_sums, ntiles, off1, cursor);
+                BZK_LAUNCHED(ctx);
+                k_round_fwd<F><<<rnd_blocks, kRoundThreads, fsm, st>>>(d_bases, scr, acc_list, acc_off, off1, pl.TB, rpre, thr_pre, thr_suf, blk_tot);
+                BZK_LAUNCHED(ctx);
+                k_round_mid<F><<<1, mid_threads, msm_, st>>>(blk_tot, rnd_blocks, blk_pre, blk_suf, inv_total);
+                BZK_LAUNCHED(ctx);
+                k_round_bwd<F><<<rnd_blocks, kRoundThreads, 0, st>>>(d_bases, scr, scr_base, acc_list, acc_off, off1, pl.TB, rpre, thr_pre, thr_suf, blk_pre,
+                                                                     blk_suf, inv_total, list1);
+                BZK_LAUNCHED(ctx);
+                scr_base += (uint32_t)cap[r + 1];
+                acc_list = list1;
+                acc_off = off1;
+            }
+        }
+        if (streamed) BZK_CUDA(ctx, cudaStreamWaitEvent(st, pipe->ready[cb], 0));
+        // the first pass fills the buckets; later ones fill the cleared pass array, folded in below
+        Xyzz<F> *target = pass ? pass_buckets : buckets;
+        if (pass) BZK_CUDA(ctx, cudaMemsetAsync(pass_buckets, 0, (size_t)pl.TB * sizeof(Xyzz<F>), st));
+        k_accumulate<F><<<acc_blocks, 128, 0, st>>>(d_bases, R ? scr : nullptr, acc_list, acc_off, pl.TB, 16u, target, part_pts, part_bucket);
+        BZK_LAUNCHED(ctx);
+        timing_mark(ctx);
+        BZK_CUDA(ctx, cudaMemsetAsync(long_len, 0, 16, st));
+        k_fixup<F><<<div_up(nslots, 128), 128, 0, st>>>(part_pts, part_bucket, nslots, acc_off, pl.TB, acc_blocks * 128, 16u, target, long_queue, long_len);
+        BZK_LAUNCHED(ctx);
+        k_fixup_long<F><<<ctx->sm_count, 256, fsmem, st>>>(part_pts, part_bucket, target, long_queue, long_len);
+        BZK_LAUNCHED(ctx);
+        if (streamed) BZK_CUDA(ctx, cudaEventRecord(pipe->freed[cb], st));  // the chunk buffer is free for chunk pass + 2
+        if (pass) {
+            k_bucket_fold<F><<<div_up(pl.TB, 128), 128, 0, st>>>(buckets, pass_buckets, pl.TB);
+            BZK_LAUNCHED(ctx);
+        }
     }
     timing_mark(ctx);
     k_bucket_slices<F><<<div_up(nslices, 128), 128, 0, st>>>(buckets, pl.NB, slice, nslices, slice_acc, slice_run);
@@ -800,7 +892,8 @@ static int32_t msm_run(bzk_ctx *ctx, const BasesRef<F> &d_bases, const Fr *d_sca
     Xyzz<F> h_win[kMaxWinPoints];
     MsmPlan pl;
     uint32_t *d_long_len = nullptr;
-    BZK_TRY(msm_enqueue<F>(ctx, ctx->stream, &ctx->ws, &ctx->ws_bytes, true, d_bases, d_scalars, n, h_win, &pl, &d_long_len));
+    BZK_TRY(msm_enqueue<F>(ctx, ctx->stream, &ctx->ws, &ctx->ws_bytes, &ctx->pipe[0], true, d_bases, d_scalars, n, h_win, &pl, &d_long_len,
+                           ctx->last_stream));
     // the plan this call ran (bzk_ctx_last_msm_plan); the queue length costs a copy, so only with timing on
     uint32_t long_len = 0;
     if (ctx->timing && d_long_len) BZK_CUDA(ctx, cudaMemcpyAsync(&long_len, d_long_len, sizeof long_len, cudaMemcpyDeviceToHost, ctx->stream));

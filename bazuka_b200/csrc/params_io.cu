@@ -16,6 +16,9 @@
 // decode kernels write the packed Montgomery points straight into the key's resident base vectors, so device memory
 // beyond the key is the two chunks.  A refused point is reported through one atomicMin over (vector, index, reason): the
 // first bad point in file order wins.  The writer runs the same pipeline backwards (encode kernel, D2H, host copy).
+// A vector placed in host memory (bzk_groth16_params_read_placed) is decoded into a device landing chunk that is then
+// copied, on the same stream, into the vector's pinned allocation; the writer copies such a vector's chunks to the device
+// before it encodes them.  Device memory is then the pipe's buffers, the landing chunk and the device-placed vectors.
 #include "common.cuh"
 #include "params_io.cuh"
 #include <algorithm>
@@ -226,10 +229,11 @@ int32_t bzk_groth16_params_file_info(const uint8_t *bytes, size_t len, bzk_param
     return BZK_OK;
 }
 
-int32_t bzk_groth16_params_read(bzk_ctx *ctx, const uint8_t *bytes, size_t len, int32_t checked, bzk_g1_affine *alpha_g1, bzk_g1_affine *beta_g1,
-                                bzk_g2_affine *beta_g2, bzk_g2_affine *gamma_g2, bzk_g1_affine *delta_g1, bzk_g2_affine *delta_g2, bzk_g1_affine *ic,
-                                size_t ic_cap, bzk_groth16_params **out) {
-    if (!ctx || !out || (len && !bytes) || !alpha_g1 || !beta_g1 || !beta_g2 || !gamma_g2 || !delta_g1 || !delta_g2) return BZK_ERR_BAD_ARG;
+int32_t bzk_groth16_params_read_placed(bzk_ctx *ctx, const uint8_t *bytes, size_t len, int32_t checked, bzk_g1_affine *alpha_g1,
+                                       bzk_g1_affine *beta_g1, bzk_g2_affine *beta_g2, bzk_g2_affine *gamma_g2, bzk_g1_affine *delta_g1,
+                                       bzk_g2_affine *delta_g2, bzk_g1_affine *ic, size_t ic_cap, uint32_t host_mask, bzk_groth16_params **out) {
+    if (!ctx || !out || (len && !bytes) || !alpha_g1 || !beta_g1 || !beta_g2 || !gamma_g2 || !delta_g1 || !delta_g2 || host_mask > 31)
+        return BZK_ERR_BAD_ARG;
     *out = nullptr;
     BZK_CUDA(ctx, cudaSetDevice(ctx->device));
     Seg seg[kSegs];
@@ -247,34 +251,40 @@ int32_t bzk_groth16_params_read(bzk_ctx *ctx, const uint8_t *bytes, size_t len, 
         return BZK_ERR_CUDA;
     }
 
-    // destinations: the five resident vectors, and a scratch block for the verifying key's points
+    // destinations: the five vectors (device or pinned host memory, as host_mask says), and a scratch block for the
+    // verifying key's points and the landing chunk of the host-placed vectors
     bzk_g1_bases *g1v[4] = {nullptr, nullptr, nullptr, nullptr};
     bzk_g2_bases *b2 = nullptr;
     void *scratch = nullptr;
     auto release = [&]() {
         cudaStreamSynchronize(ctx->stream);
-        for (auto *b : g1v) if (b) { if (b->d) cudaFree(b->d); delete b; }
-        if (b2) { if (b2->d) cudaFree(b2->d); delete b2; }
+        for (auto *b : g1v) if (b) bases_release(b);
+        if (b2) bases_release(b2);
         if (scratch) cudaFree(scratch);
     };
     int32_t st = BZK_OK;
     const uint64_t n_ic = seg[kIc].n;
-    const size_t scratch_bytes = 256 + 3 * sizeof(G1Affine) + 3 * sizeof(G2Affine) + (n_ic ? n_ic : 1) * sizeof(G1Affine) + 3 * 256;
+    const size_t landing_bytes = host_mask ? (size_t)kChunk * sizeof(G2Affine) : 0;
+    const size_t scratch_bytes = 256 + 3 * sizeof(G1Affine) + 3 * sizeof(G2Affine) + (n_ic ? n_ic : 1) * sizeof(G1Affine) + landing_bytes + 4 * 256;
     cudaError_t e = cudaMalloc(&scratch, scratch_bytes);
-    for (int v = 0; v < 4 && e == cudaSuccess; v++) {
+    if (e != cudaSuccess) {
+        st = set_cuda_err(ctx, e, "cudaMalloc(proving key)", __FILE__, __LINE__);
+        release();
+        return st;
+    }
+    for (int v = 0; v < 4 && st == BZK_OK; v++) {
         g1v[v] = new (std::nothrow) bzk_g1_bases();
         if (!g1v[v]) { release(); return BZK_ERR_OOM; }
         g1v[v]->n = seg[kH + v].n;
-        e = cudaMalloc(&g1v[v]->d, (g1v[v]->n ? g1v[v]->n : 1) * sizeof(G1Affine));
+        st = bases_alloc(ctx, g1v[v], (host_mask >> v) & 1);
     }
-    if (e == cudaSuccess) {
+    if (st == BZK_OK) {
         b2 = new (std::nothrow) bzk_g2_bases();
         if (!b2) { release(); return BZK_ERR_OOM; }
         b2->n = seg[kBG2].n;
-        e = cudaMalloc(&b2->d, (b2->n ? b2->n : 1) * sizeof(G2Affine));
+        st = bases_alloc(ctx, b2, (host_mask >> 4) & 1);
     }
-    if (e != cudaSuccess) {
-        st = set_cuda_err(ctx, e, "cudaMalloc(proving key)", __FILE__, __LINE__);
+    if (st != BZK_OK) {
         release();
         return st;
     }
@@ -283,7 +293,9 @@ int32_t bzk_groth16_params_read(bzk_ctx *ctx, const uint8_t *bytes, size_t len, 
     G1Affine *d_vk1 = cv.take<G1Affine>(3);  // alpha, beta, delta
     G2Affine *d_vk2 = cv.take<G2Affine>(3);  // beta, gamma, delta
     G1Affine *d_ic = cv.take<G1Affine>(n_ic ? n_ic : 1);
-    void *dst[kSegs] = {d_vk1, d_vk1 + 1, d_vk2, d_vk2 + 1, d_vk1 + 2, d_vk2 + 2, d_ic, g1v[0]->d, g1v[1]->d, g1v[2]->d, g1v[3]->d, b2->d};
+    char *landing = cv.take<char>(landing_bytes);
+    auto place = [](auto *b) { return b->h ? (void *)b->h : (void *)b->d; };
+    void *dst[kSegs] = {d_vk1, d_vk1 + 1, d_vk2, d_vk2 + 1, d_vk1 + 2, d_vk2 + 2, d_ic, place(g1v[0]), place(g1v[1]), place(g1v[2]), place(g1v[3]), place(b2)};
 
     {
         Pipe pipe(ctx);
@@ -293,11 +305,17 @@ int32_t bzk_groth16_params_read(bzk_ctx *ctx, const uint8_t *bytes, size_t len, 
             if (e != cudaSuccess) st = set_cuda_err(ctx, e, "cudaMemsetAsync", __FILE__, __LINE__);
         }
         for (int s = 0; s < kSegs && st == BZK_OK; s++) {
-            const size_t pb = seg_point_bytes(s);
+            const size_t pb = seg_point_bytes(s), packed = seg_is_g2(s) ? sizeof(G2Affine) : sizeof(G1Affine);
+            const bool on_host = s >= kH && ((host_mask >> (s - kH)) & 1);
             for (uint64_t i = 0; i < seg[s].n && st == BZK_OK; i += kChunk) {
                 const uint32_t n = (uint32_t)std::min<uint64_t>(kChunk, seg[s].n - i);
-                char *d = (char *)dst[s] + i * (seg_is_g2(s) ? sizeof(G2Affine) : sizeof(G1Affine));
-                st = pipe.decode(bytes + seg[s].off + i * pb, s, i, n, checked != 0, *k, d, d_fault);
+                char *d = (char *)dst[s] + i * packed;
+                st = pipe.decode(bytes + seg[s].off + i * pb, s, i, n, checked != 0, *k, on_host ? landing : d, d_fault);
+                // the landing chunk's next decode is behind this copy on the same stream
+                if (st == BZK_OK && on_host) {
+                    e = cudaMemcpyAsync(d, landing, n * packed, cudaMemcpyDeviceToHost, ctx->stream);
+                    if (e != cudaSuccess) st = set_cuda_err(ctx, e, "cudaMemcpyAsync(host vector)", __FILE__, __LINE__);
+                }
             }
         }
     }  // the pipe synchronises both streams and releases its buffers
@@ -335,6 +353,12 @@ int32_t bzk_groth16_params_read(bzk_ctx *ctx, const uint8_t *bytes, size_t len, 
     return st;
 }
 
+int32_t bzk_groth16_params_read(bzk_ctx *ctx, const uint8_t *bytes, size_t len, int32_t checked, bzk_g1_affine *alpha_g1, bzk_g1_affine *beta_g1,
+                                bzk_g2_affine *beta_g2, bzk_g2_affine *gamma_g2, bzk_g1_affine *delta_g1, bzk_g2_affine *delta_g2, bzk_g1_affine *ic,
+                                size_t ic_cap, bzk_groth16_params **out) {
+    return bzk_groth16_params_read_placed(ctx, bytes, len, checked, alpha_g1, beta_g1, beta_g2, gamma_g2, delta_g1, delta_g2, ic, ic_cap, 0, out);
+}
+
 int32_t bzk_groth16_params_write(bzk_ctx *ctx, const bzk_groth16_params *params, const bzk_g2_affine *gamma_g2, const bzk_g1_affine *ic, size_t n_ic,
                                  uint8_t *out, size_t cap, size_t *len) {
     if (!ctx || !params || !gamma_g2 || (n_ic && !ic) || !len) return BZK_ERR_BAD_ARG;
@@ -363,12 +387,22 @@ int32_t bzk_groth16_params_write(bzk_ctx *ctx, const bzk_groth16_params *params,
     G2Affine vk2[3] = {params->beta_g2, from_wire(gamma_g2), params->delta_g2};
     vk1[0] = params->alpha_g1; vk1[1] = params->beta_g1; vk1[2] = params->delta_g1;
     for (size_t i = 0; i < n_ic; i++) vk1[3 + i] = from_wire(ic + i);
+    // ... and a host-resident vector's chunks through a landing chunk on the device
+    const bool any_host = params->h->h || params->l->h || params->a->h || params->b1->h || params->b2->h;
+    const size_t landing_bytes = any_host ? (size_t)kChunk * sizeof(G2Affine) : 0;
     void *scratch = nullptr;
-    BZK_CUDA(ctx, cudaMalloc(&scratch, vk1.size() * sizeof(G1Affine) + sizeof vk2 + 256));
-    G1Affine *d_vk1 = (G1Affine *)scratch;
-    G2Affine *d_vk2 = (G2Affine *)((char *)scratch + ((vk1.size() * sizeof(G1Affine) + 255) & ~(size_t)255));
+    Carver sizer(nullptr);
+    sizer.take<G1Affine>(vk1.size()); sizer.take<G2Affine>(3); sizer.take<char>(landing_bytes);
+    BZK_CUDA(ctx, cudaMalloc(&scratch, sizer.used()));
+    Carver cv(scratch);
+    G1Affine *d_vk1 = cv.take<G1Affine>(vk1.size());
+    G2Affine *d_vk2 = cv.take<G2Affine>(3);
+    char *landing = cv.take<char>(landing_bytes);
+    auto place = [](const auto *b) { return b->h ? (const void *)b->h : (const void *)b->d; };
     const void *src[kSegs] = {d_vk1, d_vk1 + 1, d_vk2, d_vk2 + 1, d_vk1 + 2, d_vk2 + 2, d_vk1 + 3,
-                              params->h->d, params->l->d, params->a->d, params->b1->d, params->b2->d};
+                              place(params->h), place(params->l), place(params->a), place(params->b1), place(params->b2)};
+    const bool seg_host[kSegs] = {false, false, false, false, false, false, false,
+                                  params->h->h != nullptr, params->l->h != nullptr, params->a->h != nullptr, params->b1->h != nullptr, params->b2->h != nullptr};
     int32_t st = BZK_OK;
     cudaError_t e = cudaMemcpyAsync(d_vk1, vk1.data(), vk1.size() * sizeof(G1Affine), cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_vk2, vk2, sizeof vk2, cudaMemcpyHostToDevice, ctx->stream);
@@ -380,7 +414,14 @@ int32_t bzk_groth16_params_write(bzk_ctx *ctx, const bzk_groth16_params *params,
             const size_t pb = seg_point_bytes(s), packed = seg_is_g2(s) ? sizeof(G2Affine) : sizeof(G1Affine);
             for (uint64_t i = 0; i < seg[s].n && st == BZK_OK; i += kChunk) {
                 const uint32_t n = (uint32_t)std::min<uint64_t>(kChunk, seg[s].n - i);
-                st = pipe.encode((const char *)src[s] + i * packed, s, n, out + seg[s].off + i * pb);
+                const char *from = (const char *)src[s] + i * packed;
+                if (seg_host[s]) {
+                    // the previous chunk's encode kernel read the landing chunk earlier on the same stream
+                    e = cudaMemcpyAsync(landing, from, n * packed, cudaMemcpyHostToDevice, ctx->stream);
+                    if (e != cudaSuccess) { st = set_cuda_err(ctx, e, "cudaMemcpyAsync(host vector)", __FILE__, __LINE__); break; }
+                    from = landing;
+                }
+                st = pipe.encode(from, s, n, out + seg[s].off + i * pb);
             }
         }
         if (st == BZK_OK) st = pipe.drain();

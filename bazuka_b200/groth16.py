@@ -178,9 +178,30 @@ def _upload_r1cs(ctx, r1cs):
     return h
 
 
+KEY_VECTORS = ("h", "l", "a", "b_g1", "b_g2")
+
+
+def host_mask(host_vectors):
+    """names from KEY_VECTORS (or "all") -> the bit mask of bzk_groth16_params_move / _read_placed"""
+    if isinstance(host_vectors, str):
+        host_vectors = KEY_VECTORS if host_vectors == "all" else (host_vectors,)
+    mask = 0
+    for name in host_vectors or ():
+        if name not in KEY_VECTORS:
+            raise ValueError(f"unknown key vector {name!r}; expected one of {KEY_VECTORS}")
+        mask |= 1 << KEY_VECTORS.index(name)
+    return mask
+
+
 class ProvingKey:
     def __init__(self, ctx, handle, vk):
         self._ctx, self._h, self.vk = ctx, handle, vk
+
+    def move(self, host_mask):
+        """place the five vectors: bit v of host_mask (KEY_VECTORS order) set = pinned host memory, clear = device memory
+        (bzk_groth16_params_move).  Host vectors are streamed to the device by every proof; proofs are unchanged."""
+        self._ctx._check(self._ctx._l.bzk_groth16_params_move(self._ctx._h, self._h, int(host_mask)))
+        return self
 
     def free(self):
         if self._h:
@@ -210,13 +231,17 @@ def proving_key_from_host(ctx, vk, h, l, a, b_g1, b_g2, table_levels=None):
     return _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels)
 
 
-def _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels=None):
+def _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels=None, host_vectors=()):
     out = ct.c_void_p()
     pts = [np.ascontiguousarray(vk[k], dtype=np.uint8) for k in ("alpha_g1", "beta_g1", "beta_g2", "delta_g1", "delta_g2")]
     ctx._check(ctx._l.bzk_groth16_params_create(ctx._h, *[_host_ptr(p) for p in pts], hb._h, lb._h, ab._h, b1b._h, b2b._h, ct.byref(out)))
     for b in (hb, lb, ab, b1b, b2b):
         b._h = None  # adopted by the params handle
-    return _with_tables(ProvingKey(ctx, out, vk), table_levels)
+    pk = ProvingKey(ctx, out, vk)
+    mask = host_mask(host_vectors)
+    if mask:
+        pk.move(mask)   # before the tables: host vectors have none
+    return _with_tables(pk, table_levels)
 
 
 def _with_tables(pk, table_levels):
@@ -257,19 +282,22 @@ def parameters_info(src):
     return {k: int(out[0][k]) for k in PARAMS_FILE_INFO.names}
 
 
-def read_parameters(ctx, src, checked=True, table_levels=None):
+def read_parameters(ctx, src, checked=True, table_levels=None, host_vectors=()):
     """bellman `Parameters::read(src, checked)` onto the GPU -> (ProvingKey, vk dict of wire images).  checked=True tests
     every point for the curve equation and the prime-order subgroup (on the GPU); the verifying key is checked either way.
-    table_levels: as in proving_key_from_host.  A refused file raises BzkError naming the first bad point."""
+    table_levels: as in proving_key_from_host (host vectors stay untabled).  host_vectors: names from KEY_VECTORS, or
+    "all", read into pinned host memory instead of the device (bzk_groth16_params_read_placed), so a key larger than the
+    device can be read.  A refused file raises BzkError naming the first bad point."""
     buf = _file_bytes(src)
     n_ic = parameters_info(buf)["n_ic"]
     g1 = {k: np.zeros(G1_BYTES, np.uint8) for k in ("alpha_g1", "beta_g1", "delta_g1")}
     g2 = {k: np.zeros(G2_BYTES, np.uint8) for k in ("beta_g2", "gamma_g2", "delta_g2")}
     ic = np.zeros((max(n_ic, 1), G1_BYTES), np.uint8)
     out = ct.c_void_p()
-    ctx._check(ctx._l.bzk_groth16_params_read(ctx._h, _host_ptr(buf), buf.size, int(bool(checked)), _host_ptr(g1["alpha_g1"]),
-                                              _host_ptr(g1["beta_g1"]), _host_ptr(g2["beta_g2"]), _host_ptr(g2["gamma_g2"]),
-                                              _host_ptr(g1["delta_g1"]), _host_ptr(g2["delta_g2"]), _host_ptr(ic), n_ic, ct.byref(out)))
+    ctx._check(ctx._l.bzk_groth16_params_read_placed(ctx._h, _host_ptr(buf), buf.size, int(bool(checked)), _host_ptr(g1["alpha_g1"]),
+                                                     _host_ptr(g1["beta_g1"]), _host_ptr(g2["beta_g2"]), _host_ptr(g2["gamma_g2"]),
+                                                     _host_ptr(g1["delta_g1"]), _host_ptr(g2["delta_g2"]), _host_ptr(ic), n_ic,
+                                                     host_mask(host_vectors), ct.byref(out)))
     vk = dict(g1, **g2, ic=ic[:n_ic])
     return _with_tables(ProvingKey(ctx, out, vk), table_levels), vk
 
@@ -549,10 +577,11 @@ def zkproof_blob(proof_bytes):
 # ------------------------------------------------------------------------------------------------
 # trusted setup on the GPU (bellman `generate_parameters`, explicit toxic waste)
 # ------------------------------------------------------------------------------------------------
-def setup_gpu(ctx: Context, r1cs, toxic, g1_image, g2_image, table_levels=None):
+def setup_gpu(ctx: Context, r1cs, toxic, g1_image, g2_image, table_levels=None, host_vectors=()):
     """toxic = [tau, alpha, beta, gamma, delta] as [5,4] Montgomery; g1/g2: generator wire images.
     Returns (ProvingKey, vk dict).  All field/group work runs in libbzk kernels; numpy only moves
-    and reorders data.  table_levels: as in proving_key_from_host.
+    and reorders data.  table_levels: as in proving_key_from_host.  host_vectors: as in read_parameters; for a
+    BlockedR1CS each such vector moves to host memory as soon as it is built, so the device holds one of them at a time.
     r1cs: an R1CS (the key keeps its wire images in pk.device_images), or a BlockedR1CS: the Lagrange columns come from
     bzk_r1cs_columns_dev, each vector is multiplied straight into its resident form and every temporary is dropped before
     the next vector is made, so the device never holds a vector twice; no wire images are kept.  Both give the same key."""
@@ -560,13 +589,13 @@ def setup_gpu(ctx: Context, r1cs, toxic, g1_image, g2_image, table_levels=None):
     # torch slicing / indexing kernels and libbzk kernels interleave below: put both on one stream
     ctx.use_torch_stream()
     try:
-        return _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels)
+        return _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels, host_vectors)
     finally:
         torch.cuda.synchronize()
         ctx.use_own_stream()
 
 
-def _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels):
+def _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels, host_vectors):
     import torch
     t = torch
     toxic = np.ascontiguousarray(toxic, dtype=np.uint64).reshape(5, 4)
@@ -616,7 +645,7 @@ def _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels):
     ctx.ntt_dev(d_pw, log_m, NTT_IFFT)                                     # d_pw <- L_j(tau)
     if isinstance(r1cs, BlockedR1CS):
         step = seg = None
-        return _setup_blocked(ctx, r1cs, toxic, g1_image, g2_image, table_levels, d_pw, h_k, dinv, ginv, dev, rep, mul, add)
+        return _setup_blocked(ctx, r1cs, toxic, g1_image, g2_image, table_levels, host_vectors, d_pw, h_k, dinv, ginv, dev, rep, mul, add)
     lag = d_pw
     cols = []
     for k in range(3):
@@ -667,12 +696,12 @@ def _setup_gpu(ctx, r1cs, toxic, g1_image, g2_image, table_levels):
     b2b = ctx.g2_bases_from_dev(b2_pts.contiguous() if len(b_idx) else t.empty((1, G2_BYTES), dtype=t.uint8, device="cuda"), len(b_idx))
     ctx.synchronize()
     host = {"h": h_pts, "l": l_pts, "a": a_pts, "b_g1": b1_pts, "b_g2": b2_pts}
-    pk = _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels)
+    pk = _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels, host_vectors)
     pk.device_images = host  # wire images kept for tests / export
     return pk, vk
 
 
-def _setup_blocked(ctx, r1cs, toxic, g1_image, g2_image, table_levels, lag, h_k, dinv, ginv, dev, rep, mul, add):
+def _setup_blocked(ctx, r1cs, toxic, g1_image, g2_image, table_levels, host_vectors, lag, h_k, dinv, ginv, dev, rep, mul, add):
     """the rest of _setup_gpu for a BlockedR1CS (lag = L_j(tau), h_k = tau^i Z(tau)/delta): the same key, built one
     resident vector at a time"""
     import torch
@@ -682,19 +711,22 @@ def _setup_blocked(ctx, r1cs, toxic, g1_image, g2_image, table_levels, lag, h_k,
     g1_image = np.ascontiguousarray(g1_image, dtype=np.uint8)
     g2_image = np.ascontiguousarray(g2_image, dtype=np.uint8)
 
-    def bases(kind, scal):
+    on_host = host_mask(host_vectors)
+
+    def bases(kind, scal, name):
         out = ct.c_void_p()
         n = scal.shape[0]
         fn = ctx._l.bzk_g1_bases_fixed_base_mul if kind == 1 else ctx._l.bzk_g2_bases_fixed_base_mul
         ctx._check(fn(ctx._h, _host_ptr(g1_image if kind == 1 else g2_image), _p(scal.contiguous()) if n else None, n, ct.byref(out)))
         ctx.synchronize()
-        return (G1Bases if kind == 1 else G2Bases)(ctx, out)
+        b = (G1Bases if kind == 1 else G2Bases)(ctx, out)
+        return b.move_to_host() if on_host & host_mask(name) else b
 
     def drop():
         torch.cuda.synchronize()
         torch.cuda.empty_cache()   # hand freed temporaries back before libbzk allocates the next vector
 
-    hb = bases(1, h_k)
+    hb = bases(1, h_k, "h")
     del h_k
     drop()
     h = _upload_r1cs(ctx, r1cs)
@@ -717,18 +749,18 @@ def _setup_blocked(ctx, r1cs, toxic, g1_image, g2_image, table_levels, lag, h_k,
     ext_l = mul(ext[ni:].contiguous(), rep(dinv, na)) if na else ext[ni:]
     del ext
     drop()
-    lb = bases(1, ext_l)
+    lb = bases(1, ext_l, "l")
     del ext_l
     drop()
     a_idx, b_idx = r1cs.density()
-    ab = bases(1, at[t.from_numpy(a_idx.astype(np.int64)).cuda()])
+    ab = bases(1, at[t.from_numpy(a_idx.astype(np.int64)).cuda()], "a")
     del at
     drop()
     bsc = bt[t.from_numpy(b_idx.astype(np.int64)).cuda()]
     del bt
     drop()
-    b1b = bases(1, bsc)
-    b2b = bases(2, bsc)
+    b1b = bases(1, bsc, "b_g1")
+    b2b = bases(2, bsc, "b_g2")
     del bsc
     drop()
 
@@ -746,7 +778,7 @@ def _setup_blocked(ctx, r1cs, toxic, g1_image, g2_image, table_levels, lag, h_k,
     vk_g2 = images(2, tox[[2, 3, 4]])      # beta, gamma, delta
     vk = {"alpha_g1": vk_g1[0], "beta_g1": vk_g1[1], "delta_g1": vk_g1[2],
           "beta_g2": vk_g2[0], "gamma_g2": vk_g2[1], "delta_g2": vk_g2[2], "ic": ic}
-    return _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels), vk
+    return _make_pk(ctx, vk, hb, lb, ab, b1b, b2b, table_levels, host_vectors), vk
 
 
 def _p(tensor):

@@ -84,6 +84,14 @@ int32_t bzk_ctx_set_msm_table_window(bzk_ctx *ctx, uint32_t c);
  * groups, buckets per group, buckets per reduction slice, bits of the slice index, and the number of bucket runs queued
  * for the CTA-wide fold (read back only while bzk_ctx_set_timing is on, else 0).  W = 0: empty sum or no MSM yet. */
 int32_t bzk_ctx_last_msm_plan(const bzk_ctx *ctx, uint32_t out[8]);
+/* Points per device chunk buffer of the sums over host-resident vectors (bzk_g*_bases_move) on this context: 0 = the
+ * library default (2^22 G1 / 2^21 G2 points, 384 MB per buffer, two buffers per sum), otherwise 256 <= points < 2^31;
+ * anything else is BZK_ERR_BAD_ARG.  Results are the same group elements for any chunk. */
+int32_t bzk_ctx_set_msm_stream_chunk(bzk_ctx *ctx, uint64_t points);
+/* How the last single MSM on this context (as bzk_ctx_last_msm_plan) used its bases: out = { chunks, points per chunk,
+ * bytes copied host->device, 1 if it streamed a host-resident vector }; all 0 for a device vector.  A streamed sum records
+ * no stage marks (bzk_ctx_stage_ms) and runs no batched-affine rounds whatever bzk_ctx_set_msm_affine_rounds says. */
+int32_t bzk_ctx_last_msm_stream(const bzk_ctx *ctx, uint64_t out[4]);
 /* kernels launched through this ctx since creation (bench.py's `gpu_launches`) */
 uint64_t bzk_ctx_launch_count(const bzk_ctx *ctx);
 
@@ -176,6 +184,18 @@ uint32_t bzk_g1_bases_levels(const bzk_g1_bases *bases);
 uint32_t bzk_g2_bases_levels(const bzk_g2_bases *bases);
 size_t bzk_g1_bases_len(const bzk_g1_bases *b);
 size_t bzk_g2_bases_len(const bzk_g2_bases *b);
+/* Host-resident vectors, for keys that need not fit in device memory.  move(to_host != 0) puts the vector's points
+ * (level 0, packed Montgomery, 96 / 192 B each) in pinned host memory and frees its device storage, tables included;
+ * move(0) brings them back as an untabled device vector.  The context's streams, side streams included, are synchronised
+ * first; the vector is never held twice on the device.  A failed pinned allocation is BZK_ERR_OOM (the size in
+ * bzk_last_error; there is no pageable fallback) and leaves the vector where it was.  Every MSM and prover entry point
+ * takes a host vector and streams its points to the device in chunks (bzk_ctx_set_msm_stream_chunk), overlapped with the
+ * accumulation, with the same results.  precompute on a host vector is BZK_ERR_BAD_ARG; _len, _levels (1) and _free
+ * work in both places.  on_host: 1 when the vector is in host memory, else 0. */
+int32_t bzk_g1_bases_move(bzk_ctx *ctx, bzk_g1_bases *b, int32_t to_host);
+int32_t bzk_g2_bases_move(bzk_ctx *ctx, bzk_g2_bases *b, int32_t to_host);
+int32_t bzk_g1_bases_on_host(const bzk_g1_bases *b);
+int32_t bzk_g2_bases_on_host(const bzk_g2_bases *b);
 /* sum over bases[offset .. offset+n) with host scalars (copied in) or device scalars */
 int32_t bzk_msm_g1_resident(bzk_ctx *ctx, const bzk_g1_bases *b, size_t offset, const bzk_fr *scalars, size_t n, bzk_g1_affine *out);
 int32_t bzk_msm_g2_resident(bzk_ctx *ctx, const bzk_g2_bases *b, size_t offset, const bzk_fr *scalars, size_t n, bzk_g2_affine *out);
@@ -252,8 +272,13 @@ int32_t bzk_groth16_prove_dev(bzk_ctx *ctx, const bzk_groth16_params *params, co
                               bzk_g1_affine *proof_a, bzk_g2_affine *proof_b, bzk_g1_affine *proof_c);
 
 /* Fixed-base tables for the five base vectors of a key; max_levels = 0: as many levels (<= 16) as fit in
- * mem_fraction_percent % (0 = 50) of the free device memory.  See bzk_g1_bases_precompute. */
+ * mem_fraction_percent % (0 = 50) of the free device memory.  See bzk_g1_bases_precompute.  Host-resident vectors are
+ * left untabled. */
 int32_t bzk_groth16_params_precompute(bzk_ctx *ctx, bzk_groth16_params *params, uint32_t max_levels, uint32_t mem_fraction_percent);
+/* Places each of the key's five vectors: bit v of host_mask (order h, l, a, b_g1, b_g2) set = pinned host memory, clear =
+ * device memory (bzk_g1_bases_move; the moves to the host run first).  host_mask > 31 is BZK_ERR_BAD_ARG.  A key may mix
+ * both; every prover entry point gives the same proofs for any placement. */
+int32_t bzk_groth16_params_move(bzk_ctx *ctx, bzk_groth16_params *params, uint32_t host_mask);
 
 /* Proving keys as bellman 0.14 keeps them on disk: the image `Parameters::write` makes and `Parameters::read` takes
  * (layout in csrc/params_io.cu).  Points stream through two fixed staging chunks into the key's resident vectors, so
@@ -274,6 +299,15 @@ int32_t bzk_groth16_params_read(bzk_ctx *ctx, const uint8_t *bytes, size_t len, 
                                 bzk_g1_affine *alpha_g1, bzk_g1_affine *beta_g1, bzk_g2_affine *beta_g2, bzk_g2_affine *gamma_g2,
                                 bzk_g1_affine *delta_g1, bzk_g2_affine *delta_g2, bzk_g1_affine *ic, size_t ic_cap,
                                 bzk_groth16_params **out);
+/*   read_placed  read with each vector placed where host_mask says: bit v (order h, l, a, b_g1, b_g2) set = the vector
+ *              goes to pinned host memory (bzk_g1_bases_move) through a device landing chunk, so a key larger than the
+ *              device can be read, checked; device memory is then the staging chunks and the device-placed vectors.
+ *              host_mask > 31 is BZK_ERR_BAD_ARG.  Refusals as for read; nothing stays allocated, pinned memory
+ *              included.  read is read_placed with host_mask = 0.  write takes host vectors too. */
+int32_t bzk_groth16_params_read_placed(bzk_ctx *ctx, const uint8_t *bytes, size_t len, int32_t checked,
+                                       bzk_g1_affine *alpha_g1, bzk_g1_affine *beta_g1, bzk_g2_affine *beta_g2, bzk_g2_affine *gamma_g2,
+                                       bzk_g1_affine *delta_g1, bzk_g2_affine *delta_g2, bzk_g1_affine *ic, size_t ic_cap,
+                                       uint32_t host_mask, bzk_groth16_params **out);
 int32_t bzk_groth16_params_write(bzk_ctx *ctx, const bzk_groth16_params *params, const bzk_g2_affine *gamma_g2,
                                  const bzk_g1_affine *ic, size_t n_ic, uint8_t *out, size_t cap, size_t *len);
 
