@@ -45,20 +45,36 @@ static Fr host_root_of_unity(uint32_t log_n) {
     return w;
 }
 
+// both tables are built into locals and published together: `tb.d_fwd` set means both tables are there.  A failed
+// allocation or launch (out of memory on a shared card) frees what was allocated, so a later call retries from scratch
+// instead of reading the inverse twiddles through a null pointer.
 static int32_t ensure_tables(bzk_ctx *ctx, uint32_t log_n) {
     NttTables &tb = ctx->ntt[log_n];
     if (tb.d_fwd) return BZK_OK;
     size_t half = log_n ? ((size_t)1 << (log_n - 1)) : 1;
     Fr w = host_root_of_unity(log_n);
     Fr wi = w.inv();
-    BZK_CUDA(ctx, cudaMalloc(&tb.d_fwd, half * sizeof(Fr)));
-    BZK_CUDA(ctx, cudaMalloc(&tb.d_inv, half * sizeof(Fr)));
-    const uint32_t run = 32;
-    uint32_t blocks = div_up(div_up(half, run), 128);
-    k_powers<<<blocks, 128, 0, ctx->stream>>>(w, tb.d_fwd, half, run);
-    BZK_LAUNCHED(ctx);
-    k_powers<<<blocks, 128, 0, ctx->stream>>>(wi, tb.d_inv, half, run);
-    BZK_LAUNCHED(ctx);
+    Fr *fwd = nullptr, *inv = nullptr;
+    cudaError_t e = cudaMalloc(&fwd, half * sizeof(Fr));
+    if (e == cudaSuccess) {
+        e = cudaMalloc(&inv, half * sizeof(Fr));
+        if (e == cudaSuccess) {
+            const uint32_t run = 32;
+            uint32_t blocks = div_up(div_up(half, run), 128);
+            k_powers<<<blocks, 128, 0, ctx->stream>>>(w, fwd, half, run);
+            k_powers<<<blocks, 128, 0, ctx->stream>>>(wi, inv, half, run);
+            ctx->launches += 2;
+            e = cudaGetLastError();  // a failed launch stays the last error even if the one after it succeeds
+            if (e != cudaSuccess) cudaFree(inv);
+        }
+        if (e != cudaSuccess) cudaFree(fwd);
+    }
+    if (e != cudaSuccess) {
+        cudaGetLastError();  // reported here: the retry's launch check must not find it again
+        return set_cuda_err(ctx, e, "ntt twiddle tables", __FILE__, __LINE__);
+    }
+    tb.d_fwd = fwd;
+    tb.d_inv = inv;
     tb.log_n = log_n;
     return BZK_OK;
 }
