@@ -35,9 +35,16 @@ struct bzk_groth16_pvk {
 
 namespace {
 
-// a proof's three points lie on their curves (the identity counts as on them)
+// a coordinate must be sent as its canonical Montgomery image (< p): x + p still fits in 384 bits and the field
+// arithmetic would read it as x, so one proof would have a second byte string (bellman's decoders refuse it too)
+BZK_HD bool canonical(const Fp &v) { return Fp::reduce_once(v) == v; }
+BZK_HD bool canonical(const G1Affine &p) { return canonical(p.x) && canonical(p.y); }
+BZK_HD bool canonical(const G2Affine &p) { return canonical(p.x.c0) && canonical(p.x.c1) && canonical(p.y.c0) && canonical(p.y.c1); }
+
+// a proof's three points are canonically encoded and lie on their curves (the identity counts as on them)
 bool on_curves(const G1Affine &A, const G2Affine &B, const G1Affine &C) {
-    return (A.is_inf() || on_curve(A)) && (B.is_inf() || on_curve(B)) && (C.is_inf() || on_curve(C));
+    return (A.is_inf() || (canonical(A) && on_curve(A))) && (B.is_inf() || (canonical(B) && on_curve(B))) &&
+           (C.is_inf() || (canonical(C) && on_curve(C)));
 }
 bzk_g1_affine g1_at(const uint8_t *p) { bzk_g1_affine g; memset(&g, 0, sizeof g); memcpy(&g, p, 97); return g; }
 bzk_g2_affine g2_at(const uint8_t *p) { bzk_g2_affine g; memset(&g, 0, sizeof g); memcpy(&g, p, 193); return g; }
@@ -181,8 +188,9 @@ __global__ void __launch_bounds__(64) k_verify_miller(const uint8_t *__restrict_
     G2Affine B = p[97 + 192] ? G2Affine::inf() : G2Affine{Fp2{rd_fp(p + 97), rd_fp(p + 145)}, Fp2{rd_fp(p + 193), rd_fp(p + 241)}};
     G1Affine C = p[290 + 96] ? G1Affine::inf() : G1Affine{rd_fp(p + 290), rd_fp(p + 338)};
     const Fp four = Fp::from_u32(4);
-    const bool okA = A.is_inf() || A.y.sqr() == A.x.sqr() * A.x + four, okC = C.is_inf() || C.y.sqr() == C.x.sqr() * C.x + four,
-               okB = B.is_inf() || B.y.sqr() == B.x.sqr() * B.x + Fp2{four, four};
+    const bool okA = A.is_inf() || (canonical(A) && A.y.sqr() == A.x.sqr() * A.x + four),
+               okC = C.is_inf() || (canonical(C) && C.y.sqr() == C.x.sqr() * C.x + four),
+               okB = B.is_inf() || (canonical(B) && B.y.sqr() == B.x.sqr() * B.x + Fp2{four, four});
     malformed[j] = (okA && okB && okC) ? 0 : 1;
     Fr r = load_vec(r_canon + j);
     auto mul127 = [&](const G1Affine &P) {
