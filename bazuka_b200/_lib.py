@@ -133,6 +133,7 @@ SIGNATURES = {
     "bzk_mpn_state_commit_accounts": (_i32, [_vp]),
     "bzk_mpn_state_shape": (_i32, [_vp, _vp]),
     "bzk_mpn_state_delta": (_i32, [_vp, _vp, ct.POINTER(_vp), ct.POINTER(_sz), ct.POINTER(_u64)]),
+    "bzk_mpn_state_apply_delta": (_i32, [_vp, _vp, _vp, _sz, _vp, ct.POINTER(_u64), ct.POINTER(_u64)]),
     "bzk_mpn_update_witness": (_i32, [_vp, _vp, _vp, _u64, _u32, _u64, _u64, _vp, _vp, _u32, _vp, _vp, _vp]),
     "bzk_mpn_work_decode": (_i32, [_vp, _sz, ct.POINTER(_vp), _vp]),
     "bzk_mpn_work_free": (_i32, [_vp]),

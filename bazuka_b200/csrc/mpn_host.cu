@@ -11,12 +11,30 @@
 // operands, `bazuka_b200/mpn/witness_program.py::raw_values`), the state root entering every slot, and the three
 // state-dependent public inputs.  Scalars cross the ABI as canonical 32-byte little-endian integers.
 #include "common.cuh"
+#include "hash_plan.cuh"
 #include "mpn_wire.cuh"
 #include <algorithm>
+#include <cstdarg>
+#include <functional>
 #include <map>
 #include <set>
+#include <string>
 #include <unordered_map>
 #include <vector>
+
+#if !defined(__CUDACC__)
+// A host compile of this file (the CPU test tier builds the ledger's host code with g++ over a host stand-in of the batched
+// Poseidon launch, bzk_poseidon_hash) has no kernels: there a plan step gathers its rows by hash_plan.cuh's per-node rule and
+// hashes them in one bzk_poseidon_hash call.  libbzk is compiled by nvcc and runs k_poseidon_plan_step (poseidon.cu) instead.
+namespace bzk {
+int32_t poseidon_plan_step(bzk_ctx *ctx, uint32_t arity, const uint32_t *ops, size_t n, const Fr *prev, const Fr *host, Fr *out) {
+    if (arity != 2 && arity != 4 && arity != 5) return BZK_ERR_BAD_ARG;
+    std::vector<Fr> rows(n * arity);
+    for (size_t k = 0; k < n * arity; k++) rows[k] = *plan_operand(ops[k], prev, host);
+    return n ? bzk_poseidon_hash(ctx, arity, (const bzk_fr *)rows.data(), n, (bzk_fr *)out) : BZK_OK;
+}
+}  // namespace bzk
+#endif
 
 namespace bzk {
 int32_t tree4_versioned_update(bzk_ctx *ctx, uint32_t depth, const uint32_t *d_tree_id, const uint64_t *d_idx, size_t n, Fr *d_vals,
@@ -514,6 +532,296 @@ int32_t bzk_mpn_state_commit_accounts(bzk_mpn_state *s) {
         s->account_count = std::max(s->account_count, kv.second + 1);
     }
     s->pending.clear();
+    return BZK_OK;
+}
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------
+// A block's `ZkDeltaPairs` applied to the ledger (DESIGN.md §3.12): decode and validate every entry, fold the entries into
+// the final accounts, plan the re-hash of every touched token tree, account leaf and state-tree node (which nodes are dirty
+// does not depend on any hash), run the plan as one launch per level, check the result, and only then write the ledger.
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+struct DeltaLeaf {
+    uint64_t acc;
+    uint32_t sub;    // 0..3: account scalar; 4 + 2 * slot + k: the token slot's id (k = 0) or balance (k = 1)
+    uint64_t entry;  // position in the image
+    Fr v;            // Montgomery
+};
+
+int32_t refuse(bzk_ctx *ctx, const char *fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(ctx->err, sizeof ctx->err, fmt, ap);
+    va_end(ap);
+    return BZK_ERR_BAD_ARG;
+}
+std::string loc_str(const uint64_t *loc, uint64_t n) {
+    std::string o = "[";
+    for (uint64_t k = 0; k < n; k++) o += (k ? ", " : "") + std::to_string(loc[k]);
+    return o + "]";
+}
+std::string loc_str(uint64_t acc, uint32_t sub) {
+    const uint64_t loc[4] = {acc, sub < 4 ? sub : 4, (sub - 4) >> 1, (sub - 4) & 1};
+    return loc_str(loc, sub < 4 ? 2 : 4);
+}
+std::string fr_hex(const Fr &a) {
+    const Fr c = a.from_mont();
+    char b[68] = "0x";
+    for (int i = 7; i >= 0; i--) snprintf(b + 2 + 8 * (7 - i), 9, "%08x", c.l[i]);
+    return b;
+}
+bool fits_u64(const Fr &a, uint64_t *out) {
+    const Fr c = a.from_mont();
+    for (int i = 2; i < 8; i++)
+        if (c.l[i]) return false;
+    *out = (uint64_t)c.l[0] | ((uint64_t)c.l[1] << 32);
+    return true;
+}
+bool is_empty(const Account &a) { return !a.tx_nonce && !a.withdraw_nonce && a.ax.is_zero() && a.ay.is_zero() && a.tokens.empty(); }
+
+// bincode of ZkDeltaPairs -> leaves sorted by (account, leaf); refuses what the MPN state model cannot address
+int32_t decode_delta(bzk_ctx *ctx, const bzk_mpn_state *s, const uint8_t *bytes, size_t len, std::vector<DeltaLeaf> &out) {
+    wire::Reader r(bytes, len);
+    const uint64_t n = r.u64();
+    if (!r.ok) return refuse(ctx, "delta image of %zu bytes is truncated before its entry count", len);
+    if (n > (len - 8) / 9) return refuse(ctx, "delta image of %zu bytes is truncated: it announces %llu entries", len, (unsigned long long)n);
+    out.reserve(n);
+    for (uint64_t e = 0; e < n; e++) {
+        const unsigned long long ee = e;
+        const uint64_t L = r.u64();
+        if (r.ok && L != 2 && L != 4) return refuse(ctx, "entry %llu: a locator of %llu elements is not a scalar of the MPN state", ee, (unsigned long long)L);
+        uint64_t loc[4] = {0, 0, 0, 0};
+        for (uint64_t k = 0; k < L && r.ok; k++) loc[k] = r.u64();
+        const uint8_t tag = r.u8();
+        if (!r.ok) return refuse(ctx, "entry %llu: delta image truncated", ee);
+        if (tag > 1) return refuse(ctx, "entry %llu: option tag %u is neither None (0) nor Some (1)", ee, tag);
+        const std::string ls = loc_str(loc, L);
+        Fr v = Fr::zero();
+        if (tag == 1) {
+            const uint8_t *p = r.take(32);
+            if (!p) return refuse(ctx, "entry %llu: delta image truncated", ee);
+            bzk_fr raw;
+            memcpy(&raw, p, 32);
+            if (!canonical(raw)) return refuse(ctx, "entry %llu: the scalar of locator %s is not canonical", ee, ls.c_str());
+            memcpy(v.l, p, 32);
+        }
+        if (loc[0] >> (2 * s->A)) return refuse(ctx, "entry %llu: locator %s outside the state tree (4^%u accounts)", ee, ls.c_str(), s->A);
+        uint32_t sub;
+        if (L == 2) {
+            if (loc[1] > 3) return refuse(ctx, "entry %llu: locator %s is not an account scalar", ee, ls.c_str());
+            sub = (uint32_t)loc[1];
+        } else {
+            if (loc[1] != 4 || loc[3] > 1) return refuse(ctx, "entry %llu: locator %s is not a token leaf", ee, ls.c_str());
+            if (loc[2] >> (2 * s->T)) return refuse(ctx, "entry %llu: locator %s outside the token tree", ee, ls.c_str());
+            sub = 4 + 2 * (uint32_t)loc[2] + (uint32_t)loc[3];
+        }
+        out.push_back(DeltaLeaf{loc[0], sub, e, v});
+    }
+    if (r.o != len) return refuse(ctx, "delta image has %zu trailing bytes after its %llu entries", len - r.o, (unsigned long long)n);
+    std::sort(out.begin(), out.end(), [](const DeltaLeaf &a, const DeltaLeaf &b) { return a.acc != b.acc ? a.acc < b.acc : a.sub < b.sub; });
+    for (size_t k = 1; k < out.size(); k++)
+        if (out[k].acc == out[k - 1].acc && out[k].sub == out[k - 1].sub) {
+            const DeltaLeaf &a = out[k - 1].entry < out[k].entry ? out[k - 1] : out[k], &b = out[k - 1].entry < out[k].entry ? out[k] : out[k - 1];
+            return refuse(ctx, "entry %llu: duplicate locator %s (entry %llu)", (unsigned long long)b.entry, loc_str(b.acc, b.sub).c_str(),
+                          (unsigned long long)a.entry);
+        }
+    return BZK_OK;
+}
+
+// one account's leaves after the delta, as an Account; refuses values the account model cannot hold
+int32_t fold_account(bzk_ctx *ctx, const Account &before, const DeltaLeaf *d, size_t n, Account *after, bool *has_x, bool *has_y) {
+    const uint64_t acc = d[0].acc;
+    Account a = before;
+    std::map<uint32_t, std::pair<Fr, Fr>> slots;   // slot -> (id, balance) for every slot the old account or the delta holds
+    for (auto &kv : before.tokens) slots[kv.first] = {kv.second.token_id, fr_from_u64(kv.second.amount)};
+    *has_x = *has_y = false;
+    for (size_t k = 0; k < n; k++) {
+        const DeltaLeaf &l = d[k];
+        uint64_t u = 0;
+        if ((l.sub == 0 || l.sub == 1 || (l.sub >= 4 && (l.sub & 1))) && !fits_u64(l.v, &u))
+            return refuse(ctx, "entry %llu: the value of locator %s does not fit in 64 bits", (unsigned long long)l.entry, loc_str(acc, l.sub).c_str());
+        switch (l.sub) {
+            case 0: a.tx_nonce = u; break;
+            case 1: a.withdraw_nonce = u; break;
+            case 2: a.ax = l.v; *has_x = true; break;
+            case 3: a.ay = l.v; *has_y = true; break;
+            default: {
+                auto &sl = slots[(l.sub - 4) >> 1];
+                ((l.sub & 1) ? sl.second : sl.first) = l.v;
+            }
+        }
+    }
+    a.tokens.clear();
+    for (auto &kv : slots) {
+        uint64_t amount = 0;
+        fits_u64(kv.second.second, &amount);
+        if (kv.second.first.is_zero()) {
+            // `Account::tokens` drops a zero-id slot: a balance there could not be reproduced by the ledger
+            if (amount) return refuse(ctx, "account %llu: token slot %u holds balance %llu under token id zero", (unsigned long long)acc, kv.first,
+                                      (unsigned long long)amount);
+            continue;
+        }
+        a.tokens[kv.first] = Money{kv.second.first, amount};
+    }
+    *after = a;
+    return BZK_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+/* See include/bzk.h. */
+int32_t bzk_mpn_state_apply_delta(bzk_ctx *ctx, bzk_mpn_state *s, const uint8_t *delta, size_t len, const bzk_fr *expect_hash,
+                                  const uint64_t *expect_size, uint64_t *n_entries) {
+    if (!ctx) return BZK_ERR_BAD_ARG;
+    if (!s || (!delta && len)) return refuse(ctx, "null ledger or delta");
+    if (!s->pending.empty())
+        return refuse(ctx, "the ledger holds %zu accounts of an unapplied prepare_works fork: apply a block's delta to the chain's ledger", s->pending.size());
+    if (expect_hash && !canonical(*expect_hash)) return refuse(ctx, "expect_hash is not canonical");
+    const uint32_t A = s->A, T = s->T;
+    // ---------------------------------------------------------------- decode, fold, index
+    std::vector<DeltaLeaf> leaves;
+    BZK_TRY(decode_delta(ctx, s, delta, len, leaves));
+    struct Touched { uint64_t idx; const Account *before; Account after; };
+    std::vector<Touched> touched;
+    std::vector<std::pair<std::pair<FrKey, FrKey>, uint64_t>> addrs;   // `index_mpn_accounts`: (x, y) of every index whose x and y both change
+    uint64_t size = s->state_size, count = s->account_count;
+    static const Account kEmpty;
+    for (size_t k = 0; k < leaves.size();) {
+        size_t e = k;
+        while (e < leaves.size() && leaves[e].acc == leaves[k].acc) e++;
+        const uint64_t idx = leaves[k].acc;
+        auto it = s->accounts.find(idx);
+        Touched t{idx, it == s->accounts.end() ? &kEmpty : &it->second, Account()};
+        bool hx = false, hy = false;
+        BZK_TRY(fold_account(ctx, *t.before, leaves.data() + k, e - k, &t.after, &hx, &hy));
+        if (hx != hy)
+            return refuse(ctx, "account %llu: the delta sets its %s but not its %s (an inconsistent account index)", (unsigned long long)idx,
+                          hx ? "x" : "y", hx ? "y" : "x");
+        if (hx) {
+            // ascending indices: one equal to the count extends it, one above it is a gap (apply_tx/mod.rs:43-51)
+            if (idx == count) count++;
+            else if (idx > count)
+                return refuse(ctx, "account %llu: a new address above the account count %llu", (unsigned long long)idx, (unsigned long long)count);
+            addrs.emplace_back(std::make_pair(key_of(t.after.ax), key_of(t.after.ay)), idx);
+        }
+        size += leaf_count(t.after) - leaf_count(*t.before);
+        touched.push_back(std::move(t));
+        k = e;
+    }
+    // ---------------------------------------------------------------- the plan: one step per tree level, values on the host
+    // hv = tdefaults[0..T] ++ defaults[0..A] ++ the leaf scalars and clean siblings the plan reads
+    std::vector<Fr> hv(s->tdefaults);
+    hv.insert(hv.end(), s->defaults.begin(), s->defaults.end());
+    auto host = [&](const Fr &v) { hv.push_back(v); return kPlanHost | (uint32_t)(hv.size() - 1); };
+    struct Step { uint32_t arity; size_t ops_off, out_off, n; };
+    std::vector<Step> steps;
+    std::vector<uint32_t> ops;
+    size_t n_out = 0;
+    auto close_step = [&](uint32_t arity, size_t ops_off) {
+        const size_t n = (ops.size() - ops_off) / arity;
+        steps.push_back(Step{arity, ops_off, n_out, n});
+        n_out += n;
+    };
+    using Node = std::pair<uint32_t, uint64_t>;   // (touched account, node index); level lists stay sorted
+    // the parents of the nodes of `cur`, in order; a child not in `cur` is clean: clean(child) gives its operand
+    auto level = [&](std::vector<Node> &cur, const std::function<uint32_t(const Node &)> &clean) {
+        const size_t off = ops.size();
+        std::vector<Node> next;
+        for (size_t i = 0; i < cur.size();) {
+            const Node p{cur[i].first, cur[i].second >> 2};
+            for (uint64_t k = 0; k < 4; k++) {
+                const Node c{p.first, p.second * 4 + k};
+                ops.push_back(i < cur.size() && cur[i] == c ? (uint32_t)i++ : clean(c));
+            }
+            next.push_back(p);
+        }
+        close_step(4, off);
+        cur.swap(next);
+    };
+    // token trees, rebuilt from the final slots: Poseidon-2 leaves, then T levels over default siblings
+    std::vector<Node> cur;
+    {
+        const size_t off = ops.size();
+        for (size_t o = 0; o < touched.size(); o++)
+            for (auto &kv : touched[o].after.tokens) {
+                ops.push_back(host(kv.second.token_id));
+                ops.push_back(host(fr_from_u64(kv.second.amount)));
+                cur.emplace_back((uint32_t)o, kv.first);
+            }
+        close_step(2, off);
+    }
+    for (uint32_t l = 1; l <= T; l++) level(cur, [&](const Node &) { return kPlanHost | (l - 1); });
+    std::vector<uint32_t> troot(touched.size(), kPlanHost | T);
+    for (size_t i = 0; i < cur.size(); i++) troot[cur[i].first] = (uint32_t)i;
+    // account leaves: Poseidon-5(tx_nonce, withdraw_nonce, x, y, token root); an empty account hashes to defaults[0]
+    cur.clear();
+    {
+        const size_t off = ops.size();
+        for (size_t o = 0; o < touched.size(); o++) {
+            const Account &a = touched[o].after;
+            for (const Fr &v : {fr_from_u64(a.tx_nonce), fr_from_u64(a.withdraw_nonce), a.ax, a.ay}) ops.push_back(host(v));
+            ops.push_back(troot[o]);
+            cur.emplace_back(0u, touched[o].idx);
+        }
+        close_step(5, off);
+    }
+    const size_t first_state = steps.size() - 1;
+    std::vector<std::vector<uint64_t>> lvl_idx(A + 1);
+    for (auto &c : cur) lvl_idx[0].push_back(c.second);
+    for (uint32_t l = 1; l <= A; l++) {
+        level(cur, [&](const Node &c) {
+            auto it = s->levels[l - 1].find(c.second);
+            return it == s->levels[l - 1].end() ? kPlanHost | (T + l) : host(it->second);   // defaults[l - 1] sits at T + 1 + l - 1
+        });
+        for (auto &c : cur) lvl_idx[l].push_back(c.second);
+    }
+    if (hv.size() >= kPlanHost || n_out >= kPlanHost) return refuse(ctx, "delta of %zu leaves is too large for one plan", leaves.size());
+    // ---------------------------------------------------------------- enqueue every step, then one copy back
+    std::vector<Fr> res(n_out - steps[first_state].out_off);
+    if (!touched.empty()) {
+        BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+        const size_t o_hv = (ops.size() * 4 + 255) & ~(size_t)255, o_out = o_hv + ((hv.size() * sizeof(Fr) + 255) & ~(size_t)255),
+                     total = o_out + n_out * sizeof(Fr);
+        BZK_TRY(ensure_ws(ctx, &ctx->ws, &ctx->ws_bytes, total));
+        char *b = (char *)ctx->ws;
+        const uint32_t *d_ops = (const uint32_t *)b;
+        const Fr *d_hv = (const Fr *)(b + o_hv);
+        Fr *d_out = (Fr *)(b + o_out);
+        BZK_CUDA(ctx, cudaMemcpyAsync(b, ops.data(), ops.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+        BZK_CUDA(ctx, cudaMemcpyAsync(b + o_hv, hv.data(), hv.size() * sizeof(Fr), cudaMemcpyHostToDevice, ctx->stream));
+        for (size_t k = 0; k < steps.size(); k++)
+            if (steps[k].n)
+                BZK_TRY(poseidon_plan_step(ctx, steps[k].arity, d_ops + steps[k].ops_off, steps[k].n, k ? d_out + steps[k - 1].out_off : nullptr, d_hv,
+                                           d_out + steps[k].out_off));
+        BZK_CUDA(ctx, cudaMemcpyAsync(res.data(), d_out + steps[first_state].out_off, res.size() * sizeof(Fr), cudaMemcpyDeviceToHost, ctx->stream));
+        BZK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    }
+    // ---------------------------------------------------------------- check, then commit
+    const Fr root = touched.empty() ? s->node(A, 0) : res.back();
+    if ((expect_hash && !(root == fr_from_canon(expect_hash))) || (expect_size && size != *expect_size)) {
+        const std::string got = fr_hex(root), want = expect_hash ? fr_hex(fr_from_canon(expect_hash)) : std::string("any");
+        return refuse(ctx, "the delta gives state (%s, size %llu), expected (%s, size %s)", got.c_str(), (unsigned long long)size, want.c_str(),
+                      expect_size ? std::to_string(*expect_size).c_str() : "any");
+    }
+    size_t r = 0;
+    for (uint32_t l = 0; l <= A; l++)
+        for (uint64_t idx : lvl_idx[l]) s->put(l, idx, res[r++]);
+    for (auto &t : touched) {
+        if (is_empty(t.after)) s->accounts.erase(t.idx);
+        else s->accounts[t.idx] = std::move(t.after);
+    }
+    for (auto &a : addrs) {   // the reference's index is never pruned and `.first()` is the smallest index holding an address
+        auto it = s->by_addr.find(a.first);
+        if (it == s->by_addr.end()) s->by_addr.emplace(a.first, a.second);
+        else it->second = std::min(it->second, a.second);
+    }
+    s->account_count = count;
+    s->state_size = size;
+    if (n_entries) *n_entries = leaves.size();
     return BZK_OK;
 }
 

@@ -12,6 +12,7 @@
 // then MDS rows) is staged into shared memory once per CTA and read as warp-uniform broadcasts.
 // Bound: integer ALU (t=5: 1 888 Fr products per 160 B of traffic) — see DESIGN.md.
 #include "common.cuh"
+#include "hash_plan.cuh"
 
 namespace bzk {
 
@@ -48,26 +49,22 @@ __device__ __forceinline__ Fr mds_row_dot(const Fr *__restrict__ m_scaled, const
     return Fr::redc_wide(acc);
 }
 
-// Register-resident state, fully unrolled lanes (T <= 9).
+// The constant table of width T (round constants, the MDS matrix, the MDS rows pre-scaled by 2^32) staged into shared
+// memory by the whole CTA.
 template <int T>
-__global__ void __launch_bounds__(128) k_poseidon_reg(const Fr *__restrict__ consts, uint32_t rf, uint32_t rp,
-                                                      const Fr *__restrict__ in, size_t n, Fr *__restrict__ out) {
-    extern __shared__ uint4 smem_raw[];
-    Fr *sc = (Fr *)smem_raw;
+__device__ __forceinline__ void stage_consts(const Fr *__restrict__ consts, uint32_t rf, uint32_t rp, Fr *sc) {
     const uint32_t nconst = T * (rf + rp) + 2 * T * T;
-    {
-        const uint4 *src = (const uint4 *)consts;
-        uint4 *dst = (uint4 *)sc;
-        for (uint32_t i = threadIdx.x; i < nconst * 2; i += blockDim.x) dst[i] = src[i];
-    }
+    const uint4 *src = (const uint4 *)consts;
+    uint4 *dst = (uint4 *)sc;
+    for (uint32_t i = threadIdx.x; i < nconst * 2; i += blockDim.x) dst[i] = src[i];
     __syncthreads();
+}
+
+// The permutation on a register-resident state over the staged table: R_F/2 full rounds, R_P partial rounds, R_F/2 full
+// rounds; the digest is s[1].
+template <int T>
+__device__ __forceinline__ void poseidon_rounds(Fr (&s)[T], const Fr *sc, uint32_t rf, uint32_t rp) {
     const Fr *mds = sc + T * (rf + rp) + T * T;  // rows pre-scaled by 2^32 for the lazy row product
-    size_t h = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (h >= n) return;
-    Fr s[T];
-    s[0] = Fr::zero();
-#pragma unroll
-    for (int i = 1; i < T; i++) s[i] = load_vec(in + h * (T - 1) + (i - 1));
     const uint32_t half = rf / 2;
     const Fr *rc = sc;
 #pragma unroll 1
@@ -87,6 +84,22 @@ __global__ void __launch_bounds__(128) k_poseidon_reg(const Fr *__restrict__ con
 #pragma unroll
         for (int i = 0; i < T; i++) s[i] = o[i];
     }
+}
+
+// Register-resident state, fully unrolled lanes (T <= 9).
+template <int T>
+__global__ void __launch_bounds__(128) k_poseidon_reg(const Fr *__restrict__ consts, uint32_t rf, uint32_t rp,
+                                                      const Fr *__restrict__ in, size_t n, Fr *__restrict__ out) {
+    extern __shared__ uint4 smem_raw[];
+    Fr *sc = (Fr *)smem_raw;
+    stage_consts<T>(consts, rf, rp, sc);
+    size_t h = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= n) return;
+    Fr s[T];
+    s[0] = Fr::zero();
+#pragma unroll
+    for (int i = 1; i < T; i++) s[i] = load_vec(in + h * (T - 1) + (i - 1));
+    poseidon_rounds<T>(s, sc, rf, rp);
     store_vec(out + h, s[1]);
 }
 
@@ -173,19 +186,11 @@ __global__ void __launch_bounds__(128) k_merkle4_root(const Fr *__restrict__ con
     constexpr int T = 5;
     extern __shared__ uint4 smem_raw[];
     Fr *sc = (Fr *)smem_raw;
-    const uint32_t nconst = T * (rf + rp) + 2 * T * T;
-    {
-        const uint4 *src = (const uint4 *)consts;
-        uint4 *dst = (uint4 *)sc;
-        for (uint32_t i = threadIdx.x; i < nconst * 2; i += blockDim.x) dst[i] = src[i];
-    }
-    __syncthreads();
-    const Fr *mds = sc + T * (rf + rp) + T * T;
+    stage_consts<T>(consts, rf, rp, sc);
     const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= m) return;
     Fr cur = load_vec(leaves + p);
     uint64_t index = idx[p];
-    const uint32_t half = rf / 2;
     for (uint32_t lvl = 0; lvl < log4; lvl++) {
         const uint32_t pos = (uint32_t)(index & 3);
         index >>= 2;
@@ -198,24 +203,7 @@ __global__ void __launch_bounds__(128) k_merkle4_root(const Fr *__restrict__ con
             if ((uint32_t)k == pos) s[1 + k] = cur;
             else s[1 + k] = load_vec(sib + (w++));
         }
-        const Fr *rc = sc;
-#pragma unroll 1
-        for (uint32_t rnd = 0; rnd < rf + rp; rnd++) {
-#pragma unroll
-            for (int i = 0; i < T; i++) s[i] = s[i] + lds_fr(rc + i);
-            rc += T;
-            if (rnd < half || rnd >= half + rp) {
-#pragma unroll
-                for (int i = 0; i < T; i++) s[i] = pow5(s[i]);
-            } else {
-                s[0] = pow5(s[0]);
-            }
-            Fr o[T];
-#pragma unroll
-            for (int j = 0; j < T; j++) o[j] = mds_row_dot<T>(mds + j * T, s);
-#pragma unroll
-            for (int i = 0; i < T; i++) s[i] = o[i];
-        }
+        poseidon_rounds<T>(s, sc, rf, rp);
         cur = s[1];
     }
     store_vec(roots + p, cur);
@@ -245,14 +233,7 @@ __global__ void __launch_bounds__(128) k_tree4_versioned_level(const Fr *__restr
     constexpr int T = 5;
     extern __shared__ uint4 smem_raw[];
     Fr *sc = (Fr *)smem_raw;
-    const uint32_t nconst = T * (rf + rp) + 2 * T * T;
-    {
-        const uint4 *src = (const uint4 *)consts;
-        uint4 *dst = (uint4 *)sc;
-        for (uint32_t i = threadIdx.x; i < nconst * 2; i += blockDim.x) dst[i] = src[i];
-    }
-    __syncthreads();
-    const Fr *mds = sc + T * (rf + rp) + T * T;
+    stage_consts<T>(consts, rf, rp, sc);
     const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n) return;
     const Fr *cur = vals + (size_t)lvl * n;
@@ -290,25 +271,7 @@ __global__ void __launch_bounds__(128) k_tree4_versioned_level(const Fr *__restr
         for (int k = 0; k < 4; k++)
             if ((uint32_t)k != pos) store_vec(po + (w++), s[1 + k]);
     }
-    const uint32_t half = rf / 2;
-    const Fr *rc = sc;
-#pragma unroll 1
-    for (uint32_t rnd = 0; rnd < rf + rp; rnd++) {
-#pragma unroll
-        for (int i = 0; i < T; i++) s[i] = s[i] + lds_fr(rc + i);
-        rc += T;
-        if (rnd < half || rnd >= half + rp) {
-#pragma unroll
-            for (int i = 0; i < T; i++) s[i] = pow5(s[i]);
-        } else {
-            s[0] = pow5(s[0]);
-        }
-        Fr o[T];
-#pragma unroll
-        for (int j = 0; j < T; j++) o[j] = mds_row_dot<T>(mds + j * T, s);
-#pragma unroll
-        for (int i = 0; i < T; i++) s[i] = o[i];
-    }
+    poseidon_rounds<T>(s, sc, rf, rp);
     store_vec(vals + (size_t)(lvl + 1) * n + e, s[1]);
 }
 
@@ -381,6 +344,49 @@ int32_t poseidon_launch(bzk_ctx *ctx, uint32_t arity, const Fr *d_in, size_t n, 
     k_poseidon_gen<<<div_up(n, threads), threads, smem, ctx->stream>>>(pt.d_consts, T, pt.rf, pt.rp, d_in, n, d_out);
     BZK_LAUNCHED(ctx);
     return BZK_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// One step of a hash plan (hash_plan.cuh): one thread per output node; each operand comes from the previous step's outputs
+// or from the plan's host-supplied values, as its tag says.  bzk_mpn_state_apply_delta runs a block's whole re-hash as a
+// chain of these, one per tree level, with no host round trip in between.
+// ---------------------------------------------------------------------------------------------
+template <int T>
+__global__ void __launch_bounds__(128) k_poseidon_plan_step(const Fr *__restrict__ consts, uint32_t rf, uint32_t rp, const uint32_t *__restrict__ ops,
+                                                            size_t n, const Fr *__restrict__ prev, const Fr *__restrict__ host, Fr *__restrict__ out) {
+    extern __shared__ uint4 smem_raw[];
+    Fr *sc = (Fr *)smem_raw;
+    stage_consts<T>(consts, rf, rp, sc);
+    const size_t h = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= n) return;
+    Fr s[T];
+    s[0] = Fr::zero();
+#pragma unroll
+    for (int i = 1; i < T; i++) s[i] = load_vec(plan_operand(ops[h * (T - 1) + (i - 1)], prev, host));
+    poseidon_rounds<T>(s, sc, rf, rp);
+    store_vec(out + h, s[1]);
+}
+
+template <int T>
+static int32_t launch_plan_step(bzk_ctx *ctx, const uint32_t *d_ops, size_t n, const Fr *d_prev, const Fr *d_host, Fr *d_out) {
+    const PoseidonTable &pt = ctx->pos[T];
+    const size_t smem = (size_t)(pt.nrc + 2 * T * T) * sizeof(Fr);
+    BZK_CUDA(ctx, cudaFuncSetAttribute(k_poseidon_plan_step<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_poseidon_plan_step<T><<<div_up(n, 128), 128, smem, ctx->stream>>>(pt.d_consts, pt.rf, pt.rp, d_ops, n, d_prev, d_host, d_out);
+    BZK_LAUNCHED(ctx);
+    return BZK_OK;
+}
+
+int32_t poseidon_plan_step(bzk_ctx *ctx, uint32_t arity, const uint32_t *d_ops, size_t n, const Fr *d_prev, const Fr *d_host, Fr *d_out) {
+    if (!ctx->pos_loaded) return BZK_ERR_NO_PARAMS;
+    if (n && (!d_ops || !d_host || !d_out)) return BZK_ERR_BAD_ARG;
+    if (n == 0) return BZK_OK;
+    switch (arity) {
+        case 2: return launch_plan_step<3>(ctx, d_ops, n, d_prev, d_host, d_out);
+        case 4: return launch_plan_step<5>(ctx, d_ops, n, d_prev, d_host, d_out);
+        case 5: return launch_plan_step<6>(ctx, d_ops, n, d_prev, d_host, d_out);
+        default: return BZK_ERR_BAD_ARG;
+    }
 }
 
 }  // namespace bzk

@@ -120,6 +120,29 @@ class NativeLedger:
         """the block built on this fork was applied: its new accounts enter the chain's address index"""
         self.ctx._check(self.ctx._l.bzk_mpn_state_commit_accounts(self._h))
 
+    def apply_delta(self, delta, expect=None):
+        """apply a block's MPN state delta, as a full node does (`update_contract` + `index_mpn_accounts`): `delta` is the dict
+        `works.final_delta` returns ({locator: value | None}) or its bincode (`works.enc_delta`, bzk_mpn_state_delta's image);
+        `expect` = {"state_hash", "state_size"} (either may be absent), the `ZkCompressedState` the block attested.  All or
+        nothing: a refused delta (BzkError) leaves the ledger as it was.  A snapshot is a delta from the empty ledger.
+        -> the number of entries applied."""
+        from ..api import _host_ptr
+        from . import wire as Wr
+        from .works import enc_delta
+        if isinstance(delta, dict):
+            w = Wr.Writer()
+            enc_delta(w, delta)
+            delta = bytes(w.b)
+        expect = expect or {}
+        h = expect.get("state_hash")
+        hb = np.ascontiguousarray(_canon(h)) if h is not None else None
+        size = ct.c_uint64(expect["state_size"]) if expect.get("state_size") is not None else None
+        n = ct.c_uint64()
+        delta = bytes(delta)
+        self.ctx._check(self.ctx._l.bzk_mpn_state_apply_delta(self.ctx._h, self._h, delta, len(delta), _host_ptr(hb) if hb is not None else None,
+                                                              ct.byref(size) if size is not None else None, ct.byref(n)))
+        return n.value
+
     def set_account(self, index, acc: MpnAccount):
         from ..api import _host_ptr
         idx = np.array(sorted(acc.tokens), dtype=np.uint32)

@@ -389,6 +389,26 @@ int32_t bzk_mpn_state_shape(const bzk_mpn_state *state, uint32_t out[2]);   /* {
  * Option<ZkScalar>>: [account, field] for the four account scalars, [account, 4, token slot, 0 | 1] for a token's id / balance;
  * a leaf that became zero is None.  Ascending locator order; release with bzk_buffer_free. */
 int32_t bzk_mpn_state_delta(const bzk_mpn_state *before, const bzk_mpn_state *after, uint8_t **bytes, size_t *len, uint64_t *n_entries);
+/* A block's MPN state delta applied to the ledger, as a full node does for every block (`update_contract` with
+ * `index_mpn_accounts`, /root/reference/src/blockchain/ops/apply_tx/update_contract/mod.rs:130-144).
+ *   delta        the bincode of ZkDeltaPairs, the image bzk_mpn_state_delta writes; None = the leaf becomes zero
+ *                (`v.unwrap_or_default()`, /root/reference/src/zk/state/mod.rs:285-308).  Locators [i, f] (f < 4) and
+ *                [i, 4, slot, 0 | 1] with i < 4^log4_tree, slot < 4^log4_token.  The result does not depend on entry order.
+ *   indexing     (/root/reference/src/blockchain/ops/apply_tx/mod.rs:14-56) every index whose x and y are both in the delta
+ *                records its (x, y); an address keeps its smallest index; indices equal to the account count advance it in
+ *                ascending order.  An index above the count, or x without y (or y without x), is refused.
+ *   expect_hash  canonical; with expect_size, the ZkCompressedState the block attested (update_contract/mod.rs:139-144); NULL:
+ *                no check.
+ *   n_entries    optional: the number of entries applied.
+ * All hashing runs on the context's stream as one launch per tree level and one copy back.  All or nothing: on any refusal
+ * or error the ledger is unchanged and bzk_last_error(ctx) says why.  BZK_ERR_BAD_ARG refuses a truncated image, trailing
+ * bytes, an option tag other than 0 / 1, a duplicate locator, a locator outside the MPN state model, a non-canonical scalar,
+ * a value the account model cannot hold (nonce or balance >= 2^64, a balance under token id zero), an indexing
+ * inconsistency, a root or size other than expected, and a ledger holding a prepare_works fork's new accounts (apply to the
+ * chain's ledger, not to a fork).  A snapshot is a delta too: bzk_mpn_state_delta(empty ledger, ledger) applied to a fresh
+ * ledger rebuilds it. */
+int32_t bzk_mpn_state_apply_delta(bzk_ctx *ctx, bzk_mpn_state *state, const uint8_t *delta, size_t len, const bzk_fr *expect_hash,
+                                  const uint64_t *expect_size, uint64_t *n_entries);
 /* Deposit and withdraw batches natively (`mpn::deposit::deposit`, /root/reference/src/mpn/deposit.rs:11-233; `mpn::withdraw::withdraw`,
  * /root/reference/src/mpn/withdraw.rs:10-259), next to the update builder: the same ledger, the same batched GPU hashing,
  * rows of circuit inputs out.  `bzk_mpn_deposit` / `bzk_mpn_withdraw` carry what the circuits consume of `MpnDeposit` /
