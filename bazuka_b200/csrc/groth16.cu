@@ -443,24 +443,26 @@ int32_t bzk_r1cs_upload(bzk_ctx *ctx, uint64_t num_inputs, uint64_t num_aux, uin
     const uint64_t *rp[3] = {a_rp, b_rp, c_rp};
     const uint32_t *cl[3] = {a_col, b_col, c_col};
     const bzk_fr *vl[3] = {a_val, b_val, c_val};
+    uint32_t log_m = 0;
+    while (log_m <= 28 && (1ull << log_m) < ncons + num_inputs) log_m++;
+    if (log_m > 28) return BZK_ERR_BAD_ARG;
+    // density (bellman `eval`: terms with a zero coefficient are skipped): A over aux only (all inputs are always
+    // present), B over inputs and aux; found in the same pass over the terms that checks their columns and coefficients
+    std::vector<uint8_t> a_d(nv, 0), b_d(nv, 0);
+    uint8_t *pres[3] = {a_d.data(), b_d.data(), nullptr};
     for (int s = 0; s < 3; s++) {
         if (rp[s][0] != 0) return BZK_ERR_BAD_ARG;
         for (uint64_t j = 0; j < ncons; j++) if (rp[s][j + 1] < rp[s][j]) return BZK_ERR_BAD_ARG;
         if (rp[s][ncons] && (!cl[s] || !vl[s])) return BZK_ERR_BAD_ARG;
-        for (uint64_t k = 0; k < rp[s][ncons]; k++) if (cl[s][k] >= nv) return BZK_ERR_BAD_ARG;
+        for (uint64_t k = 0; k < rp[s][ncons]; k++) {
+            const uint64_t *v = vl[s][k].l;
+            if (cl[s][k] >= nv || !fr_image_canonical(v)) return BZK_ERR_BAD_ARG;
+            if (pres[s] && (v[0] | v[1] | v[2] | v[3])) pres[s][cl[s][k]] = 1;
+        }
     }
     bzk_r1cs *r = new (std::nothrow) bzk_r1cs();
     if (!r) return BZK_ERR_OOM;
-    r->num_inputs = num_inputs; r->num_aux = num_aux; r->ncons = ncons;
-    uint64_t rows = ncons + num_inputs, m = 1;
-    while (m < rows) { m <<= 1; r->log_m++; }
-    if (r->log_m > 28) { delete r; return BZK_ERR_BAD_ARG; }
-    // density (bellman `eval`: terms with a zero coefficient are skipped): A over aux only (all
-    // inputs are always present), B over inputs and aux
-    std::vector<uint8_t> a_d(nv, 0), b_d(nv, 0);
-    auto nonzero = [](const bzk_fr &v) { return (v.l[0] | v.l[1] | v.l[2] | v.l[3]) != 0; };
-    for (uint64_t k = 0; k < a_rp[ncons]; k++) if (nonzero(a_val[k])) a_d[a_col[k]] = 1;
-    for (uint64_t k = 0; k < b_rp[ncons]; k++) if (nonzero(b_val[k])) b_d[b_col[k]] = 1;
+    r->num_inputs = num_inputs; r->num_aux = num_aux; r->ncons = ncons; r->log_m = log_m;
     std::vector<uint32_t> a_idx, b_idx;
     density_lists(num_inputs, a_d, b_d, a_idx, b_idx);
     int32_t st = BZK_OK;

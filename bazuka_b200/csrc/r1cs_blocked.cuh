@@ -203,14 +203,27 @@ inline void density_lists(uint64_t num_inputs, const std::vector<uint8_t> &a_d, 
     for (uint64_t v = 0; v < nv; v++) if (b_d[v]) b_idx.push_back((uint32_t)v);
 }
 
+// Every stored coefficient must be its canonical Montgomery image (< r).  Presence is decided on the limbs, so an image
+// >= r whose value is zero (r itself) would put its variable in a density list with an identity column, which bellman's
+// Fr cannot hold and the key file reader refuses.  v: four little-endian 64-bit limbs, compared from the top one down.
+inline bool fr_image_canonical(const uint64_t v[4]) {
+    constexpr uint64_t r[4] = {0xffffffff00000001ull, 0x53bda402fffe5bfeull, 0x3339d80809a1d805ull, 0x73eda753299d7d48ull};
+    for (int i = 3; i >= 0; i--)
+        if (v[i] != r[i]) return v[i] < r[i];
+    return false;
+}
+
 // Refuses (false) what the blocked form cannot name: a non-monotone rowptr, a missing array, an expanded column at or
-// beyond nv (every copy of a slot column, up to the last), a template that repeats with a zero stride.
+// beyond nv (every copy of a slot column, up to the last), a template that repeats with a zero stride, a coefficient
+// image >= r.
 inline bool blocked_valid(const BlockedShape &b, uint64_t nv, const uint64_t *rp, const uint32_t *col, const void *val) {
     if (!rp || rp[0] != 0) return false;
     const uint64_t n = b.stored_rows(), t0 = b.head_rows, t1 = b.head_rows + b.tmpl_rows;
     for (uint64_t r = 0; r < n; r++) if (rp[r + 1] < rp[r]) return false;
     if (rp[n] && (!col || !val)) return false;
     if (b.reps && b.var_stride == 0) return false;
+    for (uint64_t e = 0; e < rp[n]; e++)
+        if (!fr_image_canonical((const uint64_t *)val + 4 * e)) return false;
     const uint64_t last = b.reps ? b.reps - 1 : 0;
     for (uint64_t r = 0; r < n; r++) {
         const bool tmpl = r >= t0 && r < t1;

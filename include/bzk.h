@@ -225,7 +225,10 @@ int32_t bzk_fr_random_dev(bzk_ctx *ctx, uint64_t seed, size_t n, void *d_out);
  * appends the `Input(i) * 0 = 0` rows itself and derives the A/B density lists from the non-zero
  * coefficients.  Parameters are bellman's `Parameters<Bls12>` vectors: h (m-1), l (num_aux),
  * a (num_inputs + |A aux density|), b_g1 / b_g2 (|B input density| + |B aux density|), in
- * bellman's order (inputs first), identity entries already filtered out. */
+ * bellman's order (inputs first), identity entries already filtered out.
+ * A term counts as present when its coefficient image is not all-zero limbs, so every coefficient must be canonical
+ * (< r, as bellman's Fr holds it): an image >= r is BZK_ERR_BAD_ARG before anything is allocated.  Otherwise r itself
+ * would be a present zero, and its variable would get an identity column that a key file may not hold. */
 typedef struct bzk_r1cs bzk_r1cs;
 typedef struct bzk_groth16_params bzk_groth16_params;
 int32_t bzk_r1cs_upload(bzk_ctx *ctx, uint64_t num_inputs, uint64_t num_aux, uint64_t num_constraints,
@@ -244,7 +247,7 @@ int32_t bzk_r1cs_shape(const bzk_r1cs *r1cs, uint64_t out[5]);
  * The handle is an ordinary bzk_r1cs for bzk_r1cs_shape / _free and every prover entry point, with the density lists
  * bzk_r1cs_upload would derive from the expanded matrices.  BZK_ERR_BAD_ARG, before anything is allocated: a rowptr
  * that does not start at 0 or decreases, a missing array, an expanded column (the last copy's included) >= num_inputs +
- * num_aux, num_inputs + num_aux > 2^32, or var_stride = 0 with reps > 0. */
+ * num_aux, num_inputs + num_aux > 2^32, var_stride = 0 with reps > 0, or a coefficient image >= r (as bzk_r1cs_upload). */
 int32_t bzk_r1cs_upload_blocked(bzk_ctx *ctx, uint64_t num_inputs, uint64_t num_aux, uint64_t head_rows, uint64_t tmpl_rows, uint64_t reps,
                                 uint64_t tail_rows, uint64_t var_lo, uint64_t var_stride, const uint64_t *const rowptr[3], const uint32_t *const col[3],
                                 const bzk_fr *const val[3], bzk_r1cs **out);
