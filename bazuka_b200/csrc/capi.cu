@@ -176,6 +176,7 @@ int32_t bzk_ctx_destroy(bzk_ctx *ctx) {
     for (auto &p : ctx->pos) if (p.d_consts) cudaFree(p.d_consts);
     for (auto &t : ctx->ntt) { if (t.d_fwd) cudaFree(t.d_fwd); if (t.d_inv) cudaFree(t.d_inv); }
     if (ctx->d_gpow) cudaFree(ctx->d_gpow);
+    if (ctx->d_jj_table) cudaFree(ctx->d_jj_table);
     if (ctx->ws) cudaFree(ctx->ws);
     if (ctx->stage) cudaFree(ctx->stage);
     if (ctx->pinned) cudaFreeHost(ctx->pinned);

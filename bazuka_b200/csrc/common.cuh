@@ -93,6 +93,10 @@ struct bzk_ctx {
     bool g16_valid = false;
     bzk::MsmPlan g16_plan[5];            // plans of the five sums of the proof in flight (kept across bzk_groth16_shard_begin / _finish)
     bool split_open = false;        // a shard_begin is waiting for its shard_finish
+    // JubJub fixed-base table of BASE (jubjub.cuh, kJJFixedEntries JJNiels) for the curve d it was built with, made by the first
+    // batch signature check (jubjub.cu)
+    void *d_jj_table = nullptr;
+    bzk::Fr jj_table_d{};
 };
 
 // A base vector, in one of two places.  On the device, `d` holds it; after bzk_g*_bases_precompute `d` holds tab_T levels

@@ -12,6 +12,7 @@
 // state-dependent public inputs.  Scalars cross the ABI as canonical 32-byte little-endian integers.
 #include "common.cuh"
 #include "hash_plan.cuh"
+#include "jubjub.cuh"
 #include "mpn_wire.cuh"
 #include <algorithm>
 #include <cstdarg>
@@ -105,47 +106,9 @@ struct bzk_mpn_state {
             idx >>= 2;
         }
     }
-    bool on_curve(const Fr &x, const Fr &y) const {
-        Fr x2 = x * x, y2 = y * y;
-        return (y2 - x2) == (Fr::one() + jj_d * x2 * y2);
-    }
 };
 
 namespace {
-
-// Fr square root (Tonelli-Shanks, r - 1 = 2^32 * q with q odd, 7 = non-residue); false when none exists.  One 223-bit power:
-// w = a^((q-1)/2) gives both x = a*w = a^((q+1)/2) and t = x*w = a^q; the loop then corrects x by powers of c = 7^q (computed
-// once); a non-residue is recognised at the end (x^2 != a) instead of by a separate Legendre power.
-bool fr_sqrt(const Fr &a, Fr *out) {
-    if (a.is_zero()) { *out = a; return true; }
-    // q = (r - 1) >> 32, as 32-bit words (224 bits); e = (q - 1) / 2
-    uint32_t q[8] = {0}, rm1[8], e[8];
-    for (int i = 0; i < 8; i++) rm1[i] = FrParams::p(i);
-    rm1[0] -= 1;
-    for (int i = 0; i < 7; i++) q[i] = rm1[i + 1];
-    for (int i = 0; i < 8; i++) e[i] = (q[i] >> 1) | (i < 7 ? q[i + 1] << 31 : 0);   // q is odd: (q - 1) / 2 = q >> 1
-    static const Fr c0 = Fr::from_u32(7).pow(q, 8);   // generator of the 2^32-torsion
-    const Fr w = a.pow(e, 8);
-    Fr x = a * w, t = x * w, c = c0;
-    uint32_t m = 32;
-    while (!(t == Fr::one())) {
-        uint32_t i = 0;
-        Fr t2 = t;
-        while (!(t2 == Fr::one())) {
-            t2 = t2 * t2;
-            if (++i == m) return false;   // t has order 2^m: a is not a square
-        }
-        Fr b = c;
-        for (uint32_t k = 0; k + i + 1 < m; k++) b = b * b;
-        m = i;
-        c = b * b;
-        t = t * c;
-        x = x * b;
-    }
-    if (!(x * x == a)) return false;
-    *out = x;
-    return true;
-}
 
 // PointCompressed::decompress (/root/reference/src/crypto/jubjub/curve.rs:78-88); x canonical in, Montgomery out
 bool jj_decompress(bzk_mpn_state *s, const bzk_fr *x_canon, bool odd, Point *out) {
@@ -154,18 +117,14 @@ bool jj_decompress(bzk_mpn_state *s, const bzk_fr *x_canon, bool odd, Point *out
     Point p;
     if (it != s->decompress_cache.end()) p = it->second;
     else {
-        Fr x2 = x * x;
-        Fr den = Fr::one() - s->jj_d * x2;
-        if (den.is_zero()) return false;
         Fr y;
-        if (!fr_sqrt((Fr::one() + x2) * den.inv_gcd(), &y)) return false;  // a = -1
+        if (!jj_decompress_root(x, s->jj_d, &y)) return false;
         p = Point{x, y};
         if (s->decompress_cache.size() >= kDecompressCacheCap) s->decompress_cache.clear();
         s->decompress_cache[key_of(x)] = p;
     }
-    const bool y_odd = (p.y.from_mont().l[0] & 1u) != 0;
     out->x = p.x;
-    out->y = (y_odd != odd) ? p.y.neg() : p.y;
+    out->y = jj_with_parity(p.y, odd);
     return true;
 }
 
@@ -267,34 +226,12 @@ struct Forest {
 };
 
 
-// ---- JubJub on the host field arithmetic (projective twisted Edwards, a = -1): /root/reference/src/crypto/jubjub/curve.rs:90-160
-struct JJ { Fr x, y, z; };
-inline JJ jj_identity() { return JJ{Fr::zero(), Fr::one(), Fr::one()}; }
-inline JJ jj_add(const JJ &p, const JJ &q, const Fr &d) {   // unified addition (also doubles)
-    const Fr a = p.z * q.z, b = a * a, c = p.x * q.x, dd = p.y * q.y, e = d * c * dd, f = b - e, g = b + e;
-    return JJ{a * f * ((p.x + p.y) * (q.x + q.y) - c - dd), a * g * (dd + c), f * g};
-}
-inline JJ jj_mul(const Point &p, const Fr &k_canon, const Fr &d) {
-    const JJ base{p.x, p.y, Fr::one()};
-    JJ acc = jj_identity();
-    for (int i = 255; i >= 0; i--) {
-        acc = jj_add(acc, acc, d);
-        if ((k_canon.l[i >> 5] >> (i & 31)) & 1) acc = jj_add(acc, base, d);
-    }
-    return acc;
-}
-inline bool jj_equal(const JJ &p, const JJ &q) { return p.x * q.z == q.x * p.z && p.y * q.z == q.y * p.z; }
-inline Point jj_base() {   // BASE (curve.rs:146-164): x below, y = 18
-    Fr x;
-    const uint32_t l[8] = {0xec7beacau, 0x4df7b7ffu, 0xfd6c54edu, 0x2e3ebb21u, 0x0fd6cce6u, 0xf1fbf02du, 0x43ac65a6u, 0x3fd2814cu};
-    memcpy(x.l, l, 32);
-    return Point{x.to_mont(), Fr::from_u32(18)};
-}
 // `JubJub::verify` (/root/reference/src/crypto/jubjub/mod.rs:151-167) given h = Poseidon(R.x, R.y, A.x, A.y, msg) (Montgomery)
 inline bool eddsa_verify_with_h(const bzk_mpn_state *s, const Point &pk, const Point &sig_r, const Fr &sig_s_canon, const Fr &h_mont) {
-    if (!s->on_curve(pk.x, pk.y) || !s->on_curve(sig_r.x, sig_r.y)) return false;
-    const JJ lhs = jj_add(jj_mul(pk, h_mont.from_mont(), s->jj_d), JJ{sig_r.x, sig_r.y, Fr::one()}, s->jj_d);
-    return jj_equal(lhs, jj_mul(jj_base(), sig_s_canon, s->jj_d));
+    Fr bx, by;
+    jj_base(&bx, &by);
+    const JJ sB = jj_mul(jj_from_affine(bx, by), sig_s_canon, s->jj_d.dbl());
+    return jj_eddsa_check(s->jj_d, pk.x, pk.y, sig_r.x, sig_r.y, h_mont.from_mont(), sB);
 }
 
 }  // namespace
@@ -899,7 +836,7 @@ int32_t bzk::mpn_update_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn
         const Money src_token = src_before.tokens[sti];
         const bool dst_has = dst_before0.tokens.count(dti) != 0;
         if (tx.nonce != src_before.tx_nonce + 1 || !(src_before.ax == src_addr.x) || !(src_before.ay == src_addr.y) ||
-            (s->on_curve(dst_before0.ax, dst_before0.ay) && (!(dst_before0.ax == dst_addr.x) || !(dst_before0.ay == dst_addr.y))) ||
+            (jj_on_curve(dst_before0.ax, dst_before0.ay, s->jj_d) && (!(dst_before0.ax == dst_addr.x) || !(dst_before0.ay == dst_addr.y))) ||
             (dst_has && !(src_token.token_id == dst_before0.tokens[dti].token_id)) || !(src_token.token_id == amt_tok_id) ||
             src_token.amount < tx.amount)
             continue;
@@ -1107,7 +1044,7 @@ int32_t bzk::mpn_deposit_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mp
         const Fr tok = fr_from_canon(&d.token_id);
         const int ti = find_token_index(before, T, tok, true);
         if (ti < 0 || (d.src_id && rejected_srcs.count(d.src_id)) ||
-            (s->on_curve(before.ax, before.ay) && (!(before.ax == addr.x) || !(before.ay == addr.y)))) {
+            (jj_on_curve(before.ax, before.ay, s->jj_d) && (!(before.ax == addr.x) || !(before.ay == addr.y)))) {
             reject();
             continue;
         }
@@ -1515,7 +1452,7 @@ extern "C" int32_t bzk_jubjub_decompress(const bzk_fr *jubjub_d, const bzk_fr *x
     bzk_mpn_state tmp;
     tmp.jj_d = fr_from_canon(jubjub_d);
     Point p;
-    if (!jj_decompress(&tmp, x, y_is_odd != 0, &p) || !tmp.on_curve(p.x, p.y)) return BZK_ERR_NOT_ON_CURVE;
+    if (!jj_decompress(&tmp, x, y_is_odd != 0, &p) || !jj_on_curve(p.x, p.y, tmp.jj_d)) return BZK_ERR_NOT_ON_CURVE;
     fr_to_canon(out_xy + 0, p.x);
     fr_to_canon(out_xy + 1, p.y);
     return BZK_OK;

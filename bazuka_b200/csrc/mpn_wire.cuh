@@ -178,6 +178,10 @@ struct Reader {
 void enc_work(Writer &w, const Work &work);
 bool dec_work(Reader &r, Work &work);
 void enc_contract_withdraw(Writer &w, const ContractWithdraw &p);
+// `bincode::serialize(&Vec<MpnWithdraw>)` / `&Vec<MpnTransaction>` images; false on a truncated image, trailing bytes, a bad tag
+// or an unreduced scalar
+bool dec_withdraws(const uint8_t *b, size_t n, std::vector<MpnWithdraw> &out);
+bool dec_txs(const uint8_t *b, size_t n, std::vector<MpnTx> &out);
 
 // sha3-256 (FIPS 202) — `Hasher::hash` of the reference (/root/reference/src/crypto/mod.rs, sha3::Sha3_256)
 void sha3_256(const uint8_t *data, size_t len, uint8_t out[32]);

@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "ff.cuh"
+#include "jubjub.cuh"
 
 namespace bzk {
 
@@ -42,12 +43,6 @@ template <class Mem>
 BZK_HD void wit_prefetch_lc(const WitProgDev &P, int32_t l, const Mem &mem) {
     const int32_t lo = P.lc_ptr[l], hi = P.lc_ptr[l + 1];
     for (int32_t k = lo; k < hi; k++) mem.prefetch(P.lc_slot[k]);
-}
-
-BZK_HD bool jj_on_curve(const Fr &x, const Fr &y, const Fr &d) {
-    // a = -1:  y^2 - x^2 == 1 + d x^2 y^2   (/root/reference/src/crypto/jubjub/curve.rs:40-47)
-    Fr x2 = x.sqr(), y2 = y.sqr();
-    return (y2 - x2) == (Fr::one() + d * x2 * y2);
 }
 
 // op j of the program (any order that respects the data flow): code / a0..a3 / imm = its row of P.ops

@@ -454,6 +454,31 @@ int32_t bzk_jubjub_decompress(const bzk_fr *jubjub_d, const bzk_fr *x, int32_t y
  * message), accept iff h*A + R == s*BASE and A, R are on the curve.  Canonical scalars; returns 1 / 0, negative on bad arguments. */
 int32_t bzk_jubjub_eddsa_verify(const bzk_poseidon_host *hasher, const bzk_fr *jubjub_d, const bzk_fr pk_xy[2], const bzk_fr *message,
                                 const bzk_fr sig_r_xy[2], const bzk_fr *sig_s);
+/* ------------------------------------------------------------------ EdDSA signature checks in batches (device)
+ * `JubJub::verify` on many signatures at once, one thread per signature: the key decompressed as `PointCompressed::decompress`
+ * does, A and R on the curve, h = Poseidon(R.x, R.y, A.x, A.y, msg), accept iff [h] A + R == [s] BASE as points of the full
+ * curve group (h and s as plain integers below r: no reduction modulo the prime order, no cofactor clearing).  A scalar that
+ * is not canonical, or a key that does not decompress (where the reference panics), gives 0.
+ *   bzk_jubjub_eddsa_verify_batch  the message as given (canonical scalars in every field)
+ *   bzk_mpn_tx_verify_batch        `MpnTransaction::verify_signature`: msg = Poseidon(nonce, D.x, D.y, amount token, amount, fee token,
+ *                                  fee), D the decompressed destination key (0 where it does not decompress)
+ *   bzk_mpn_signatures_verify_bytes  the bincode of Vec<MpnWithdraw> (kind 1: `MpnWithdraw::verify_signature`,
+ *                                  msg = Poseidon(fingerprint(payment), nonce)) or Vec<MpnTransaction> (kind 2), the images
+ *                                  bzk_mpn_prepare_works takes; ok == NULL: only *n (the item count); cap < *n: BZK_ERR_BAD_ARG
+ * ok[i] = 1 (accept) or 0 (reject); n_ok (optional) = the number accepted.  A rejected signature is a verdict: the call returns
+ * BZK_OK.  BZK_ERR_BAD_ARG (nothing written to ok): a null pointer with n > 0, jubjub_d not canonical, kind 0 or above 2, a
+ * malformed image (truncated, trailing bytes, a bad tag, an unreduced scalar).  BZK_ERR_NO_PARAMS: the context has no Poseidon
+ * table.  Synchronous on the context's stream.  Items go through the context's arenas 2^18 at a time, so device memory stays
+ * bounded for any n; the context keeps a fixed-base table of BASE (786 KB) for the last jubjub_d it was given. */
+typedef struct {
+    bzk_fr pk_x;
+    uint8_t pk_odd, pad[7];   /* PublicKey = PointCompressed(pk_x, pk_odd) */
+    bzk_fr message, sig_rx, sig_ry, sig_s;
+} bzk_eddsa_item;             /* 168 B, canonical scalars */
+int32_t bzk_jubjub_eddsa_verify_batch(bzk_ctx *ctx, const bzk_fr *jubjub_d, const bzk_eddsa_item *items, size_t n, uint8_t *ok, uint64_t *n_ok);
+int32_t bzk_mpn_tx_verify_batch(bzk_ctx *ctx, const bzk_fr *jubjub_d, const bzk_mpn_tx *txs, size_t n, uint8_t *ok, uint64_t *n_ok);
+int32_t bzk_mpn_signatures_verify_bytes(bzk_ctx *ctx, const bzk_fr *jubjub_d, uint32_t kind, const uint8_t *bytes, size_t len, uint8_t *ok,
+                                        size_t cap, uint64_t *n, uint64_t *n_ok);
 int32_t bzk_mpn_update_build(bzk_ctx *ctx, bzk_mpn_state *state, const bzk_mpn_tx *txs, uint64_t n_txs, uint32_t log4_batch,
                              const bzk_fr *fee_token, bzk_fr *raws, bzk_fr *ext, uint8_t *accepted, bzk_fr public3[3],
                              uint64_t *n_accepted);
