@@ -255,7 +255,7 @@ int32_t bzk_mpn_signatures_verify_bytes(bzk_ctx *ctx, const bzk_fr *jubjub_d, ui
         canon_of(&o.pk_x, w.mpn_address.x); o.pk_odd = w.mpn_address.odd ? 1 : 0;
         canon_of(&o.sig_rx, w.sig.r.x); canon_of(&o.sig_ry, w.sig.r.y); canon_of(&o.sig_s, w.sig.s);
         msg2[2 * k] = wire::withdraw_fingerprint(w.payment);
-        msg2[2 * k + 1] = wire::fr_of_u64(w.nonce);
+        msg2[2 * k + 1] = fr_from_u64(w.nonce);
     }
     return verify_batch(ctx, d, Items::kEddsa, in.data(), count, msg2.data(), ok, n_ok);
 }

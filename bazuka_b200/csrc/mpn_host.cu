@@ -1,15 +1,15 @@
-// bazuka_b200 — the MPN ledger and the update transition builder as native host code over the GPU primitives.
+// bazuka_b200 — the MPN ledger and the transition builders as native host code over the GPU primitives.
 //
-// Mirrors `mpn::update::update` (/root/reference/src/mpn/update.rs:8-299) on the state model of
+// Mirrors `mpn::{update,deposit,withdraw}` (/root/reference/src/mpn/update.rs:8-299, deposit.rs, withdraw.rs) on the state model of
 // /root/reference/src/mpn/mod.rs:219-240 and /root/reference/src/zk/state/mod.rs:93-208 (account leaf =
 // Poseidon-5(tx_nonce, withdraw_nonce, pk.x, pk.y, tokens_root); token leaf = Poseidon-2(token_id, amount);
 // 4-ary sparse trees with `compress_default` defaults), but in the two-phase shape of DESIGN.md §3.7:
 //   1. ledger decisions, sequential, no hashing (acceptance rules, balances, slot choice);
 //   2. all hashing in batches on the GPU: bzk_poseidon_hash for the leaves, the versioned level-synchronous
 //      tree update (poseidon.cu) for the token forest and the state tree.
-// Output = one row of circuit inputs per slot in UpdateCircuit's allocation order (the witness program's RAW
-// operands, `bazuka_b200/mpn/witness_program.py::raw_values`), the state root entering every slot, and the three
-// state-dependent public inputs.  Scalars cross the ABI as canonical 32-byte little-endian integers.
+// Output = the reference's transition structs, what a circuit row needs besides them, and the three state-dependent
+// public inputs; the C ABI writes the rows through the circuits' writers (mpn_wire.cu).  Scalars cross the ABI as
+// canonical 32-byte little-endian integers.
 #include "common.cuh"
 #include "hash_plan.cuh"
 #include "jubjub.cuh"
@@ -52,13 +52,6 @@ struct FrKey {  // Montgomery limbs as a map key
 };
 inline FrKey key_of(const Fr &a) { FrKey k; memcpy(k.l, a.l, 32); return k; }
 inline Fr fr_from_canon(const bzk_fr *c) { Fr a; memcpy(a.l, c, 32); return a.to_mont(); }
-inline void fr_to_canon(bzk_fr *out, const Fr &a) { Fr c = a.from_mont(); memcpy(out, c.l, 32); }
-inline Fr fr_from_u64(uint64_t v) {
-    Fr a = Fr::zero();
-    a.l[0] = (uint32_t)v;
-    a.l[1] = (uint32_t)(v >> 32);
-    return a.to_mont();
-}
 
 struct Money { Fr token_id; uint64_t amount; };  // token_id in Montgomery form
 struct Account {
@@ -271,7 +264,7 @@ int32_t list_root(bzk_ctx *ctx, uint32_t arity, const std::vector<Fr> &rows, Fr 
     return BZK_OK;
 }
 
-// ---- the builders' plans as the reference's transition structs (`prepare_works` puts them on the wire)
+// ---- the builders' values as the reference's transition structs
 wire::Money wire_money(const Money &m) {
     wire::Money w;
     w.token = wire::ContractId::of_scalar(m.token_id);
@@ -280,19 +273,18 @@ wire::Money wire_money(const Money &m) {
 }
 wire::Account wire_account(const Account &a) {
     wire::Account w;
-    w.tx_nonce = (uint32_t)a.tx_nonce; w.withdraw_nonce = (uint32_t)a.withdraw_nonce;
+    w.tx_nonce = a.tx_nonce; w.withdraw_nonce = a.withdraw_nonce;
     w.address.x = a.ax; w.address.y = a.ay;
     for (auto &kv : a.tokens) w.tokens.emplace_back((uint64_t)kv.first, wire_money(kv.second));   // ascending slot order
     return w;
 }
-wire::Proof wire_proof(const Fr *p, uint32_t depth) { return wire::Proof(p, p + (size_t)depth * 3); }
 }  // namespace
 
 extern "C" {
 
 int32_t bzk_mpn_update_raw_width(uint32_t A, uint32_t T, uint32_t *n_raw) {
     if (!n_raw || A == 0 || A > 31 || T == 0 || T > 8) return BZK_ERR_BAD_ARG;
-    *n_raw = 32 + 9 * T + 6 * A;
+    *n_raw = update_raw_width(A, T);
     return BZK_OK;
 }
 
@@ -762,55 +754,154 @@ int32_t bzk_mpn_state_apply_delta(bzk_ctx *ctx, bzk_mpn_state *s, const uint8_t 
     return BZK_OK;
 }
 
-int32_t bzk_mpn_update_build(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_tx *txs, uint64_t n_txs, uint32_t log4_batch,
-                             const bzk_fr *fee_token_canon, bzk_fr *raws, bzk_fr *ext, uint8_t *accepted, bzk_fr public3[3],
-                             uint64_t *n_accepted) {
-    return bzk::mpn_update_build_impl(ctx, s, txs, n_txs, log4_batch, fee_token_canon, raws, ext, accepted, public3, n_accepted, nullptr);
-}
 }  // extern "C"
 
-int32_t bzk::mpn_update_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_tx *txs, uint64_t n_txs, uint32_t log4_batch,
-                                   const bzk_fr *fee_token_canon, bzk_fr *raws, bzk_fr *ext, uint8_t *accepted, bzk_fr public3[3],
-                                   uint64_t *n_accepted, bzk::UpdateSink *sink) {
-    if (!ctx || !s || (n_txs && !txs) || !fee_token_canon || !raws || !ext || !public3 || !n_accepted || log4_batch > 8) return BZK_ERR_BAD_ARG;
-    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
-    const uint32_t A = s->A, T = s->T;
-    const uint64_t cap = 1ull << (2 * log4_batch);
-    const uint32_t n_raw = 32 + 9 * T + 6 * A;
-    const Fr fee_token = fr_from_canon(fee_token_canon), prev_root = s->node(A, 0);
-    // ---------------------------------------------------------------- phase 1: ledger decisions on a mirror
-    struct Plan {
-        uint64_t tx, src, dst;
-        uint32_t sti, sfi, dti;
-        Account src_before, src_mid, src_after, dst_before, dst_after;
-        Money src_token, src_fee_token, dst_token;
-        Point dst_addr;
-        size_t e1, e2, e3;
-        Fr src_bal_hash, dst_bal_hash;
-    };
-    std::map<uint64_t, Account> mirror;
-    auto pending = s->pending;
-    auto index_of = [&](const Point &a, uint64_t *out) {
-        const auto key = std::make_pair(key_of(a.x), key_of(a.y));
-        auto it = s->by_addr.find(key);
+// ---------------------------------------------------------------------------------------------
+// The three transition builders (DESIGN.md §3.7): each runs its own acceptance rules over the inputs, sequentially and without
+// hashing, on a BatchCore; the core then hashes the token forest and the state tree of the whole batch in batched launches.
+// Their output is the reference's transition structs plus what a circuit row needs besides them (bzk::Built); the rows
+// themselves come from the writers of csrc/mpn_wire.cu.
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+wire::PointW null_key() { return wire::PointW{Fr::zero(), Fr::one().neg()}; }   // PublicKey::default().decompress() = (0, -1)
+
+// The ledger side of one batch.  The acceptance loop looks accounts up (index_of, next_index, get) and records every accepted
+// change as steps.  A step is one token-forest write (token `slot` of the account, as it is in `after`) and one state-tree write
+// (the leaf of `after` over the token root that write leaves); reading an account after a step sees `after`.  hash() runs both
+// trees over all steps; per step the core then gives the token root before it, its token proof, its state proof and the state
+// root after it.
+struct BatchCore {
+    bzk_mpn_state *s;
+    Fr prev_root;
+    std::map<uint64_t, Account> mirror;                    // the accounts the batch has changed
+    std::map<std::pair<FrKey, FrKey>, uint64_t> pending;   // s->pending and the accounts this batch creates
+    struct Step { uint64_t acc; uint32_t slot; Account after; };
+    std::vector<Step> steps;
+    std::vector<uint64_t> touched;                         // the steps' accounts in first-seen order
+    Forest forest;
+    std::vector<Fr> tok_root, s_vals, s_proofs;
+
+    explicit BatchCore(bzk_mpn_state *st) : s(st), prev_root(st->node(st->A, 0)), pending(st->pending) {}
+    static std::pair<FrKey, FrKey> key(const Point &a) { return std::make_pair(key_of(a.x), key_of(a.y)); }
+    // update.rs:47-70: the chain's index table first, then the accounts created earlier on this fork
+    bool index_of(const Point &a, uint64_t *out) const {
+        auto it = s->by_addr.find(key(a));
         if (it != s->by_addr.end()) { *out = it->second; return true; }
-        auto jt = pending.find(key);
+        auto jt = pending.find(key(a));
         if (jt != pending.end()) { *out = jt->second; return true; }
         return false;
-    };
-    auto get = [&](uint64_t i) -> Account {
+    }
+    // the index of an unknown address: mpn_account_count + |new_account_indices|; add_account records it
+    uint64_t next_index() const { return s->account_count + pending.size(); }
+    void add_account(const Point &a, uint64_t i) { pending.emplace(key(a), i); }
+    Account get(uint64_t i) const {
         auto it = mirror.find(i);
         if (it != mirror.end()) return it->second;
         auto jt = s->accounts.find(i);
-        Account a = jt == s->accounts.end() ? Account() : jt->second;
-        mirror[i] = a;
-        return a;
-    };
-    std::vector<Plan> plan;
+        return jt == s->accounts.end() ? Account() : jt->second;
+    }
+    void step(uint64_t acc, uint32_t slot, const Account &after) {
+        mirror[acc] = after;
+        steps.push_back(Step{acc, slot, after});
+    }
+
+    // the token forest (the touched accounts' pre-batch tokens enter as writes into empty trees, then one write per step), then
+    // the accounts' leaves and the state tree
+    int32_t hash(bzk_ctx *ctx) {
+        const uint32_t A = s->A;
+        forest.T = s->T;
+        for (auto &st : steps)
+            if (forest.tree_of.emplace(st.acc, (uint32_t)forest.tree_of.size()).second) touched.push_back(st.acc);
+        for (uint64_t acc : touched) {
+            auto it = s->accounts.find(acc);
+            if (it != s->accounts.end())
+                for (auto &kv : it->second.tokens) forest.write(acc, kv.first, kv.second);
+        }
+        forest.n_init = forest.idx.size();
+        for (auto &st : steps) forest.write(st.acc, st.slot, st.after.tokens.at(st.slot));
+        BZK_TRY(forest.run(ctx, s->tdefaults));
+        std::vector<Fr> rows;
+        rows.reserve(steps.size() * 5);
+        for (size_t k = 0; k < steps.size(); k++) {
+            const Account &a = steps[k].after;
+            tok_root.push_back(forest.root(steps[k].acc));
+            const Fr r = forest.applied(steps[k].acc, forest.n_init + k);
+            for (const Fr &v : {fr_from_u64(a.tx_nonce), fr_from_u64(a.withdraw_nonce), a.ax, a.ay, r}) rows.push_back(v);
+        }
+        BZK_TRY(hash_rows(ctx, 5, rows, s_vals));
+        const size_t ne = steps.size();
+        std::vector<uint64_t> idx(ne);
+        std::vector<Fr> init(ne * A * 3);
+        for (size_t e = 0; e < ne; e++) {
+            idx[e] = steps[e].acc;
+            s->prove(idx[e], init.data() + e * A * 3);
+        }
+        return tree_update_host(ctx, A, std::vector<uint32_t>(ne, 0u), idx, s_vals, init, s_proofs);
+    }
+    Fr tok_before(size_t k) const { return tok_root[k]; }
+    wire::Proof tok_proof(size_t k) const {
+        const Fr *p = forest.proofs.data() + (forest.n_init + k) * s->T * 3;
+        return wire::Proof(p, p + (size_t)s->T * 3);
+    }
+    wire::Proof state_proof(size_t k) const {
+        const Fr *p = s_proofs.data() + k * s->A * 3;
+        return wire::Proof(p, p + (size_t)s->A * 3);
+    }
+    Fr root_after(size_t k) const { return s_vals[(size_t)s->A * steps.size() + k]; }
+    Fr root() const { return steps.empty() ? prev_root : root_after(steps.size() - 1); }
+    // the state root entering each of `cap` slots when every transition made `per` steps; after the last one the state no longer moves
+    std::vector<Fr> slot_roots(uint64_t cap, size_t per) const {
+        std::vector<Fr> r(cap, root());
+        for (size_t k = 0; k * per < steps.size(); k++) r[k] = k ? root_after(k * per - 1) : prev_root;
+        return r;
+    }
+    // the ledger moves to the end of the batch; public3 = {state, aux_data, next_state}
+    void commit(const Fr &aux, bzk_fr public3[3]) {
+        const size_t ne = steps.size();
+        for (size_t e = 0; e < ne; e++) {
+            uint64_t node = steps[e].acc;
+            for (uint32_t l = 0; l <= s->A; l++) { s->put(l, node, s_vals[(size_t)l * ne + e]); node >>= 2; }
+        }
+        for (uint64_t i : touched) {
+            auto it = s->accounts.find(i);
+            if (it != s->accounts.end()) s->state_size -= leaf_count(it->second);
+            s->state_size += leaf_count(mirror[i]);
+            s->accounts[i] = mirror[i];
+        }
+        s->pending = pending;
+        fr_to_canon(public3 + 0, prev_root);
+        fr_to_canon(public3 + 1, aux);
+        fr_to_canon(public3 + 2, root());
+    }
+};
+
+template <class Tr>
+void report(const Built<Tr> &bt, uint64_t n_in, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted) {
+    if (accepted) {
+        memset(accepted, 0, n_in);
+        for (uint64_t k : bt.from) accepted[k] = 1;
+    }
+    memcpy(public3, bt.public3, sizeof bt.public3);
+    *n_accepted = bt.t.size();
+}
+
+}  // namespace
+
+// `mpn::update::update` (/root/reference/src/mpn/update.rs:8-299): three steps per transaction (the source's amount, the source's
+// fee, the destination)
+int32_t bzk::mpn_update_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_tx *txs, uint64_t n_txs, uint32_t log4_batch,
+                                   const bzk_fr *fee_token_canon, Built<wire::UpdateTransition> *out) {
+    if (!ctx || !s || (n_txs && !txs) || !fee_token_canon || !out || log4_batch > 8) return BZK_ERR_BAD_ARG;
+    BZK_CUDA(ctx, cudaSetDevice(ctx->device));
+    const uint32_t A = s->A, T = s->T;
+    const uint64_t cap = 1ull << (2 * log4_batch);
+    const Fr fee_token = fr_from_canon(fee_token_canon);
+    BatchCore b(s);
+    *out = Built<wire::UpdateTransition>();
+    out->d.keys.assign(cap, null_key());
     uint64_t fee_sum = 0;
-    for (uint64_t k = 0; k < n_txs; k++) {
-        if (accepted) accepted[k] = 0;
-        if (plan.size() == cap) continue;
+    for (uint64_t k = 0; k < n_txs && out->t.size() < cap; k++) {
         const bzk_mpn_tx &tx = txs[k];
         // malformed field elements cannot be put into a witness row: such a transaction is simply not eligible
         if (!canonical(tx.src_pk_x) || !canonical(tx.dst_pk_x) || !canonical(tx.amount_token_id) || !canonical(tx.fee_token_id) ||
@@ -822,14 +913,13 @@ int32_t bzk::mpn_update_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn
         Point src_addr, dst_addr;
         if (!jj_decompress(s, &tx.src_pk_x, tx.src_pk_odd != 0, &src_addr) || !jj_decompress(s, &tx.dst_pk_x, tx.dst_pk_odd != 0, &dst_addr))
             continue;
-        // update.rs:47-70: the chain's index table first, then the accounts created earlier on this fork; an unknown
-        // sender is rejected, an unknown receiver gets index  mpn_account_count + |new_account_indices|
+        // an unknown sender is rejected, an unknown receiver gets the next new index
         uint64_t src_index = 0, dst_index = 0;
-        if (!index_of(src_addr, &src_index)) continue;
-        bool dst_new = false;
-        if (!index_of(dst_addr, &dst_index)) { dst_index = s->account_count + pending.size(); dst_new = true; }
+        if (!b.index_of(src_addr, &src_index)) continue;
+        const bool dst_new = !b.index_of(dst_addr, &dst_index);
+        if (dst_new) dst_index = b.next_index();
         if (dst_index >> (2 * A)) continue;
-        Account src_before = get(src_index), dst_before0 = get(dst_index);
+        Account src_before = b.get(src_index), dst_before0 = b.get(dst_index);
         const int sti = find_token_index(src_before, T, amt_tok_id, false), dti = find_token_index(dst_before0, T, amt_tok_id, true),
                   sfi = find_token_index(src_before, T, fee_tok_id, false);
         if (sti < 0 || dti < 0 || sfi < 0) continue;
@@ -848,199 +938,71 @@ int32_t bzk::mpn_update_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn
         const Money src_fee_token = fit->second;
         Account src_after = src_mid;
         src_after.tokens[sfi].amount -= tx.fee;
-        mirror[src_index] = src_after;
-        Account dst_before = get(dst_index);
+        b.step(src_index, sti, src_mid);
+        b.step(src_index, sfi, src_after);
+        const Account dst_before = b.get(dst_index);   // after the source's steps: a transfer to oneself sees them
         Money dst_token{Fr::zero(), 0};
-        if (dst_before.tokens.count(dti)) dst_token = dst_before.tokens[dti];
+        if (dst_before.tokens.count(dti)) dst_token = dst_before.tokens.at(dti);
         Account dst_after = dst_before;
         dst_after.ax = dst_addr.x; dst_after.ay = dst_addr.y;
         if (!dst_after.tokens.count(dti)) dst_after.tokens[dti] = Money{amt_tok_id, 0};
         dst_after.tokens[dti].amount += tx.amount;
-        mirror[dst_index] = dst_after;
-        if (dst_new) pending.emplace(std::make_pair(key_of(dst_addr.x), key_of(dst_addr.y)), dst_index);
-        Plan p{};
-        p.tx = k; p.src = src_index; p.dst = dst_index; p.sti = sti; p.sfi = sfi; p.dti = dti;
-        p.src_before = src_before; p.src_mid = src_mid; p.src_after = src_after; p.dst_before = dst_before; p.dst_after = dst_after;
-        p.src_token = src_token; p.src_fee_token = src_fee_token; p.dst_token = dst_token; p.dst_addr = dst_addr;
-        plan.push_back(std::move(p));
-        if (accepted) accepted[k] = 1;
+        b.step(dst_index, dti, dst_after);
+        if (dst_new) b.add_account(dst_addr, dst_index);
+        // `UpdateTransition` (update.rs:220-247); the hashes and proofs once the batch is hashed
+        wire::UpdateTransition t;
+        t.enabled = true;
+        t.tx.nonce = tx.nonce;
+        t.tx.src = wire::PubKey{src_addr.x, tx.src_pk_odd != 0}; t.tx.dst = wire::PubKey{dst_addr.x, tx.dst_pk_odd != 0};
+        t.tx.amount = wire_money(Money{amt_tok_id, tx.amount}); t.tx.fee = wire_money(Money{fee_tok_id, tx.fee});
+        t.tx.sig.r = wire::PointW{fr_from_canon(&tx.sig_rx), fr_from_canon(&tx.sig_ry)}; t.tx.sig.s = fr_from_canon(&tx.sig_s);
+        t.src_before = wire_account(src_before); t.src_before_balance = wire_money(src_token); t.src_before_fee_balance = wire_money(src_fee_token);
+        t.src_index = src_index; t.src_token_index = sti; t.src_fee_token_index = sfi;
+        t.dst_before = wire_account(dst_before); t.dst_before_balance = wire_money(dst_token);
+        t.dst_index = dst_index; t.dst_token_index = dti;
+        out->d.keys[out->t.size()] = wire::PointW{dst_addr.x, dst_addr.y};
+        out->t.push_back(std::move(t));
+        out->from.push_back(k);
         fee_sum += tx.fee;
     }
-    // ---------------------------------------------------------------- phase 2a: token forest
-    Forest forest;
-    forest.T = T;
-    std::vector<uint64_t> touched;
-    for (auto &p : plan)
-        for (uint64_t i : {p.src, p.dst})
-            if (forest.tree_of.emplace(i, (uint32_t)forest.tree_of.size()).second) touched.push_back(i);
-    for (uint64_t acc : touched) {
-        auto it = s->accounts.find(acc);
-        if (it != s->accounts.end())
-            for (auto &kv : it->second.tokens) forest.write(acc, kv.first, kv.second);
+    BZK_TRY(b.hash(ctx));
+    for (size_t k = 0; k < out->t.size(); k++) {
+        wire::UpdateTransition &t = out->t[k];
+        t.src_before_balances_hash = b.tok_before(3 * k); t.dst_before_balances_hash = b.tok_before(3 * k + 2);
+        t.src_balance_proof = b.tok_proof(3 * k); t.src_fee_balance_proof = b.tok_proof(3 * k + 1); t.dst_balance_proof = b.tok_proof(3 * k + 2);
+        t.src_proof = b.state_proof(3 * k); t.dst_proof = b.state_proof(3 * k + 2);
     }
-    forest.n_init = forest.idx.size();
-    for (auto &p : plan) {
-        p.e1 = forest.write(p.src, p.sti, p.src_mid.tokens[p.sti]);
-        p.e2 = forest.write(p.src, p.sfi, p.src_after.tokens[p.sfi]);
-        p.e3 = forest.write(p.dst, p.dti, p.dst_after.tokens[p.dti]);
-    }
-    BZK_TRY(forest.run(ctx, s->tdefaults));
-    std::vector<Fr> acct_rows;
-    acct_rows.reserve(plan.size() * 15);
-    auto push_acct = [&](const Account &a, const Fr &tok_root) {
-        acct_rows.push_back(fr_from_u64(a.tx_nonce)); acct_rows.push_back(fr_from_u64(a.withdraw_nonce));
-        acct_rows.push_back(a.ax); acct_rows.push_back(a.ay); acct_rows.push_back(tok_root);
-    };
-    for (auto &p : plan) {
-        p.src_bal_hash = forest.root(p.src);
-        const Fr r1 = forest.applied(p.src, p.e1), r2 = forest.applied(p.src, p.e2);
-        p.dst_bal_hash = forest.root(p.dst);
-        const Fr r3 = forest.applied(p.dst, p.e3);
-        push_acct(p.src_mid, r1); push_acct(p.src_after, r2); push_acct(p.dst_after, r3);
-    }
-    // ---------------------------------------------------------------- phase 2b: state tree
-    std::vector<Fr> s_vals, s_proofs;
-    BZK_TRY(hash_rows(ctx, 5, acct_rows, s_vals));
-    std::vector<uint64_t> s_idx;
-    for (auto &p : plan) { s_idx.push_back(p.src); s_idx.push_back(p.src); s_idx.push_back(p.dst); }
-    const size_t ne = s_idx.size();
-    std::vector<Fr> init(ne * A * 3);
-    for (size_t e = 0; e < ne; e++) s->prove(s_idx[e], init.data() + e * A * 3);
-    BZK_TRY(tree_update_host(ctx, A, std::vector<uint32_t>(ne, 0u), s_idx, s_vals, init, s_proofs));
-    // ---------------------------------------------------------------- rows of circuit inputs (raw_values order)
-    const Fr null_dst_y = Fr::one().neg();  // PublicKey::default().decompress() = (0, -1)
-    Fr root = prev_root;
-    for (uint64_t slot = 0; slot < cap; slot++) {
-        bzk_fr *row = raws + slot * n_raw;
-        memset(row, 0, (size_t)n_raw * sizeof(bzk_fr));
-        size_t w = 0;
-        auto put_fr = [&](const Fr &v) { fr_to_canon(row + (w++), v); };
-        auto put_u = [&](uint64_t v) { memcpy(row + (w++), &v, 8); };
-        auto put_proof = [&](const Fr *p, uint32_t depth) { for (uint32_t i = 0; i < depth * 3; i++) put_fr(p[i]); };
-        fr_to_canon(ext + slot * 2, fee_token);
-        if (slot >= plan.size()) {
-            // the only non-zero input of a null slot: tx.dst_pub_key.decompress().y
-            fr_to_canon(row + (23 + 9 * T + 3 * A), null_dst_y);
-            fr_to_canon(ext + slot * 2 + 1, root);  // after the last real slot the state no longer moves
-            continue;
-        }
-        const Plan &p = plan[slot];
-        const bzk_mpn_tx &tx = txs[p.tx];
-        fr_to_canon(ext + slot * 2 + 1, root);
-        put_u(1); put_u(p.sti); put_u(p.sfi); put_u(p.dti);
-        put_u(p.src_before.tx_nonce); put_u(p.src_before.withdraw_nonce); put_fr(p.src_before.ax); put_fr(p.src_before.ay);
-        put_fr(p.src_bal_hash); put_fr(p.dst_bal_hash);
-        put_fr(p.src_token.token_id); put_u(p.src_token.amount);
-        put_fr(p.src_fee_token.token_id); put_u(p.src_fee_token.amount);
-        put_proof(forest.proofs.data() + p.e1 * T * 3, T);
-        put_u(tx.amount); put_u(tx.fee);
-        put_proof(forest.proofs.data() + p.e2 * T * 3, T);
-        put_u(tx.nonce); put_u(p.src); row[w++] = tx.amount_token_id; row[w++] = tx.fee_token_id;
-        put_fr(p.dst_token.token_id); put_u(p.dst_token.amount);
-        put_proof(forest.proofs.data() + p.e3 * T * 3, T);
-        put_proof(s_proofs.data() + (3 * slot) * A * 3, A);
-        put_fr(p.dst_addr.x); put_fr(p.dst_addr.y); put_u(p.dst);
-        put_u(p.dst_before.tx_nonce); put_u(p.dst_before.withdraw_nonce); put_fr(p.dst_before.ax); put_fr(p.dst_before.ay);
-        put_proof(s_proofs.data() + (3 * slot + 2) * A * 3, A);
-        row[w++] = tx.sig_rx; row[w++] = tx.sig_ry; row[w++] = tx.sig_s;
-        if (w != n_raw) return BZK_ERR_BAD_ARG;
-        root = s_vals[(size_t)A * ne + 3 * slot + 2];
-    }
-    // ---------------------------------------------------------------- commit + public inputs
-    for (size_t e = 0; e < ne; e++) {
-        uint64_t node = s_idx[e];
-        for (uint32_t l = 0; l <= A; l++) { s->put(l, node, s_vals[(size_t)l * ne + e]); node >>= 2; }
-    }
-    for (uint64_t i : touched) {
-        auto it = s->accounts.find(i);
-        if (it != s->accounts.end()) s->state_size -= leaf_count(it->second);
-        s->state_size += leaf_count(mirror[i]);
-        s->accounts[i] = mirror[i];
-    }
-    s->pending = pending;
-    std::vector<Fr> aux_in = {fee_token, fr_from_u64(fee_sum)}, aux_out;
-    BZK_TRY(hash_rows(ctx, 2, aux_in, aux_out));
-    fr_to_canon(public3 + 0, prev_root);
-    fr_to_canon(public3 + 1, aux_out[0]);
-    fr_to_canon(public3 + 2, root);
-    *n_accepted = plan.size();
-    if (sink) {   // `UpdateTransition` of every accepted transaction (/root/reference/src/mpn/update.rs:220-247)
-        sink->t.clear(); sink->from.clear();
-        for (size_t slot = 0; slot < plan.size(); slot++) {
-            const Plan &p = plan[slot];
-            wire::UpdateTransition t;
-            t.enabled = true;
-            t.src_before = wire_account(p.src_before); t.src_before_balances_hash = p.src_bal_hash;
-            t.src_before_balance = wire_money(p.src_token); t.src_before_fee_balance = wire_money(p.src_fee_token);
-            t.src_proof = wire_proof(s_proofs.data() + (3 * slot) * A * 3, A);
-            t.src_index = p.src; t.src_token_index = p.sti; t.src_balance_proof = wire_proof(forest.proofs.data() + p.e1 * T * 3, T);
-            t.src_fee_token_index = p.sfi; t.src_fee_balance_proof = wire_proof(forest.proofs.data() + p.e2 * T * 3, T);
-            t.dst_before = wire_account(p.dst_before); t.dst_before_balances_hash = p.dst_bal_hash; t.dst_before_balance = wire_money(p.dst_token);
-            t.dst_proof = wire_proof(s_proofs.data() + (3 * slot + 2) * A * 3, A);
-            t.dst_index = p.dst; t.dst_token_index = p.dti; t.dst_balance_proof = wire_proof(forest.proofs.data() + p.e3 * T * 3, T);
-            sink->t.push_back(std::move(t));
-            sink->from.push_back(p.tx);
-        }
-    }
+    out->d.roots = b.slot_roots(cap, 3);
+    std::vector<Fr> aux_in = {fee_token, fr_from_u64(fee_sum)}, aux;
+    BZK_TRY(hash_rows(ctx, 2, aux_in, aux));
+    b.commit(aux[0], out->public3);
     return BZK_OK;
 }
 
-extern "C" {
-
-
-/* `mpn::deposit::deposit` (/root/reference/src/mpn/deposit.rs:11-233) without the L1 balance bookkeeping (chain state):
- * up to 4^log4_batch eligible deposits, in order.  Outputs, one row per slot (null slots padded as DepositTransition::null):
- *   raws1[slots][5]           phase-1 inputs  {enabled, token, amount, pk.x, pk.y}
- *   raws2[slots][9+3T+3A]     phase-2 inputs  {account index, token index, account before (4), balances hash, balance before (2),
- *                             balance proof, account proof}
- *   roots[slots]              the state root entering each slot
- *   reveal[slots][4]          the rows the circuit reveals {enabled, token, amount, H(pk)}; aux_data = their list root
- *   public3                   {state, aux_data, next_state};   the ledger advances (build on a clone, see bzk_mpn_state_clone) */
-int32_t bzk_mpn_deposit_build(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_deposit *deps, uint64_t n_deps, uint32_t log4_batch, bzk_fr *raws1,
-                              bzk_fr *raws2, bzk_fr *roots, bzk_fr *reveal, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted) {
-    return bzk::mpn_deposit_build_impl(ctx, s, deps, n_deps, log4_batch, raws1, raws2, roots, reveal, accepted, public3, n_accepted, nullptr);
-}
-}  // extern "C"
-
-int32_t bzk::mpn_deposit_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_deposit *deps, uint64_t n_deps, uint32_t log4_batch, bzk_fr *raws1,
-                                    bzk_fr *raws2, bzk_fr *roots, bzk_fr *reveal, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted,
-                                    bzk::DepositSink *sink) {
-    if (!ctx || !s || (n_deps && !deps) || !raws1 || !raws2 || !roots || !reveal || !public3 || !n_accepted || log4_batch > 8) return BZK_ERR_BAD_ARG;
+// `mpn::deposit::deposit` (/root/reference/src/mpn/deposit.rs:11-233) without the L1 balance bookkeeping (chain state): one step
+// per deposit
+int32_t bzk::mpn_deposit_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_deposit *deps, uint64_t n_deps, uint32_t log4_batch,
+                                    Built<wire::DepositTransition> *out) {
+    if (!ctx || !s || (n_deps && !deps) || !out || log4_batch > 8) return BZK_ERR_BAD_ARG;
     BZK_CUDA(ctx, cudaSetDevice(ctx->device));
-    const uint32_t A = s->A, T = s->T, w2 = 9 + 3 * T + 3 * A;
+    const uint32_t A = s->A, T = s->T;
     const uint64_t cap = 1ull << (2 * log4_batch);
-    const Fr prev_root = s->node(A, 0);
-    struct Plan { uint64_t k, idx; uint32_t ti; Account before, after; Money bal; Point addr; size_t e; Fr bal_hash; };
-    std::map<uint64_t, Account> mirror;
-    auto pending = s->pending;
-    auto get = [&](uint64_t i) -> Account {
-        auto it = mirror.find(i);
-        if (it != mirror.end()) return it->second;
-        auto jt = s->accounts.find(i);
-        return jt == s->accounts.end() ? Account() : jt->second;
-    };
-    std::vector<Plan> plan;
+    BatchCore b(s);
+    *out = Built<wire::DepositTransition>();
+    out->d.keys.assign(cap, null_key());
+    std::vector<Fr> pk_rows;
     std::set<uint64_t> rejected_srcs;   // deposit.rs:33 `rejected_pub_keys`: a rejected deposit takes its L1 source's later ones with it
-    for (uint64_t k = 0; k < n_deps; k++) {
-        if (accepted) accepted[k] = 0;
-        if (plan.size() == cap) continue;
+    for (uint64_t k = 0; k < n_deps && out->t.size() < cap; k++) {
         const bzk_mpn_deposit &d = deps[k];
         auto reject = [&] { if (d.src_id) rejected_srcs.insert(d.src_id); };
         if (!canonical(d.pk_x) || !canonical(d.token_id)) { reject(); continue; }
         Point addr;
         if (!jj_decompress(s, &d.pk_x, d.pk_odd != 0, &addr)) { reject(); continue; }
-        const auto key = std::make_pair(key_of(addr.x), key_of(addr.y));
         uint64_t idx = 0;
-        bool is_new = false;
-        auto it = s->by_addr.find(key);
-        if (it != s->by_addr.end()) idx = it->second;
-        else {
-            auto jt = pending.find(key);
-            if (jt != pending.end()) idx = jt->second;
-            else { idx = s->account_count + pending.size(); is_new = true; }
-        }
+        const bool is_new = !b.index_of(addr, &idx);
+        if (is_new) idx = b.next_index();
         if (idx >> (2 * A)) { reject(); continue; }
-        const Account before = get(idx);
+        const Account before = b.get(idx);
         const Fr tok = fr_from_canon(&d.token_id);
         const int ti = find_token_index(before, T, tok, true);
         if (ti < 0 || (d.src_id && rejected_srcs.count(d.src_id)) ||
@@ -1048,133 +1010,54 @@ int32_t bzk::mpn_deposit_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mp
             reject();
             continue;
         }
-        Plan p{};
-        p.k = k; p.idx = idx; p.ti = (uint32_t)ti; p.before = before; p.addr = addr;
-        p.bal = before.tokens.count(ti) ? before.tokens.at(ti) : Money{Fr::zero(), 0};
-        p.after = before;
-        p.after.ax = addr.x; p.after.ay = addr.y;
-        if (!p.after.tokens.count(ti)) p.after.tokens[ti] = Money{tok, 0};
-        p.after.tokens[ti].amount += d.amount;
-        mirror[idx] = p.after;
-        if (is_new) pending.emplace(key, idx);
-        plan.push_back(std::move(p));
-        if (accepted) accepted[k] = 1;
+        Account after = before;
+        after.ax = addr.x; after.ay = addr.y;
+        if (!after.tokens.count(ti)) after.tokens[ti] = Money{tok, 0};
+        after.tokens[ti].amount += d.amount;
+        b.step(idx, ti, after);
+        if (is_new) b.add_account(addr, idx);
+        // `DepositTransition` (deposit.rs:150-165)
+        wire::DepositTransition t;
+        t.enabled = true;
+        t.tx.mpn_address = wire::PubKey{addr.x, d.pk_odd != 0};
+        t.tx.payment.amount = wire_money(Money{tok, d.amount});
+        t.before = wire_account(before);
+        t.before_balance = wire_money(before.tokens.count(ti) ? before.tokens.at(ti) : Money{Fr::zero(), 0});
+        t.account_index = idx; t.token_index = ti;
+        out->d.keys[out->t.size()] = wire::PointW{addr.x, addr.y};
+        pk_rows.push_back(addr.x); pk_rows.push_back(addr.y);
+        out->t.push_back(std::move(t));
+        out->from.push_back(k);
     }
-    Forest forest;
-    forest.T = T;
-    std::vector<uint64_t> touched;
-    for (auto &p : plan)
-        if (forest.tree_of.emplace(p.idx, (uint32_t)forest.tree_of.size()).second) touched.push_back(p.idx);
-    for (uint64_t acc : touched) {
-        auto it = s->accounts.find(acc);
-        if (it != s->accounts.end())
-            for (auto &kv : it->second.tokens) forest.write(acc, kv.first, kv.second);
-    }
-    forest.n_init = forest.idx.size();
-    for (auto &p : plan) p.e = forest.write(p.idx, p.ti, p.after.tokens[p.ti]);
-    BZK_TRY(forest.run(ctx, s->tdefaults));
-    std::vector<Fr> acct_rows, pk_rows;
-    for (auto &p : plan) {
-        p.bal_hash = forest.root(p.idx);
-        const Fr r = forest.applied(p.idx, p.e);
-        const Account &a = p.after;
-        acct_rows.push_back(fr_from_u64(a.tx_nonce)); acct_rows.push_back(fr_from_u64(a.withdraw_nonce));
-        acct_rows.push_back(a.ax); acct_rows.push_back(a.ay); acct_rows.push_back(r);
-        pk_rows.push_back(p.addr.x); pk_rows.push_back(p.addr.y);
-    }
-    std::vector<Fr> s_vals, s_proofs, pk_hash;
-    BZK_TRY(hash_rows(ctx, 5, acct_rows, s_vals));
+    BZK_TRY(b.hash(ctx));
+    std::vector<Fr> pk_hash;
     BZK_TRY(hash_rows(ctx, 2, pk_rows, pk_hash));
-    std::vector<uint64_t> s_idx;
-    for (auto &p : plan) s_idx.push_back(p.idx);
-    const size_t ne = s_idx.size();
-    std::vector<Fr> init(ne * A * 3);
-    for (size_t e = 0; e < ne; e++) s->prove(s_idx[e], init.data() + e * A * 3);
-    BZK_TRY(tree_update_host(ctx, A, std::vector<uint32_t>(ne, 0u), s_idx, s_vals, init, s_proofs));
-    const Fr minus_one = Fr::one().neg();
-    Fr root = prev_root;
-    std::vector<Fr> rev_rows(cap * 4, Fr::zero());
-    for (uint64_t slot = 0; slot < cap; slot++) {
-        bzk_fr *r1 = raws1 + slot * 5, *r2 = raws2 + slot * w2, *rv = reveal + slot * 4;
-        memset(r1, 0, 5 * sizeof(bzk_fr)); memset(r2, 0, (size_t)w2 * sizeof(bzk_fr)); memset(rv, 0, 4 * sizeof(bzk_fr));
-        if (slot >= plan.size()) {
-            fr_to_canon(r1 + 4, minus_one);   // PublicKey::default().decompress() = (0, -1)
-            continue;
-        }
-        const Plan &p = plan[slot];
-        const bzk_mpn_deposit &d = deps[p.k];
-        fr_to_canon(roots + slot, root);
-        uint64_t one = 1;
-        memcpy(r1 + 0, &one, 8); r1[1] = d.token_id; memcpy(r1 + 2, &d.amount, 8); fr_to_canon(r1 + 3, p.addr.x); fr_to_canon(r1 + 4, p.addr.y);
-        size_t w = 0;
-        auto put_fr = [&](const Fr &v) { fr_to_canon(r2 + (w++), v); };
-        auto put_u = [&](uint64_t v) { memcpy(r2 + (w++), &v, 8); };
-        put_u(p.idx); put_u(p.ti); put_u(p.before.tx_nonce); put_u(p.before.withdraw_nonce); put_fr(p.before.ax); put_fr(p.before.ay);
-        put_fr(p.bal_hash); put_fr(p.bal.token_id); put_u(p.bal.amount);
-        for (uint32_t i = 0; i < T * 3; i++) put_fr(forest.proofs[p.e * T * 3 + i]);
-        for (uint32_t i = 0; i < A * 3; i++) put_fr(s_proofs[slot * A * 3 + i]);
-        if (w != w2) return BZK_ERR_BAD_ARG;
-        memcpy(rv + 0, &one, 8); rv[1] = d.token_id; memcpy(rv + 2, &d.amount, 8); fr_to_canon(rv + 3, pk_hash[slot]);
-        rev_rows[slot * 4 + 0] = Fr::one(); rev_rows[slot * 4 + 1] = fr_from_canon(&d.token_id); rev_rows[slot * 4 + 2] = fr_from_u64(d.amount);
-        rev_rows[slot * 4 + 3] = pk_hash[slot];
-        root = s_vals[(size_t)A * ne + slot];
+    pk_hash.resize(cap, Fr::zero());
+    out->d.pk_hash = pk_hash;
+    for (size_t k = 0; k < out->t.size(); k++) {
+        wire::DepositTransition &t = out->t[k];
+        t.before_balances_hash = b.tok_before(k); t.balance_proof = b.tok_proof(k); t.proof = b.state_proof(k);
     }
-    for (uint64_t slot = plan.size(); slot < cap; slot++) fr_to_canon(roots + slot, root);
-    for (size_t e = 0; e < ne; e++) {
-        uint64_t node = s_idx[e];
-        for (uint32_t l = 0; l <= A; l++) { s->put(l, node, s_vals[(size_t)l * ne + e]); node >>= 2; }
-    }
-    for (uint64_t i : touched) {
-        auto it = s->accounts.find(i);
-        if (it != s->accounts.end()) s->state_size -= leaf_count(it->second);
-        s->state_size += leaf_count(mirror[i]);
-        s->accounts[i] = mirror[i];
-    }
-    s->pending = pending;
+    out->d.roots = b.slot_roots(cap, 1);
+    std::vector<wire::DepositTransition> slots;
+    padded(out->t, log4_batch, null_deposit(A, T), slots);
+    std::vector<Fr> rev(cap * 4);
+    for (uint64_t k = 0; k < cap; k++) deposit_reveal(slots[k], out->d, k, rev.data() + k * 4);
     Fr aux;
-    BZK_TRY(list_root(ctx, 4, rev_rows, &aux));
-    fr_to_canon(public3 + 0, prev_root);
-    fr_to_canon(public3 + 1, aux);
-    fr_to_canon(public3 + 2, root);
-    *n_accepted = plan.size();
-    if (sink) {   // `DepositTransition` of every accepted deposit (/root/reference/src/mpn/deposit.rs:150-165)
-        sink->t.clear(); sink->from.clear();
-        for (size_t slot = 0; slot < plan.size(); slot++) {
-            const Plan &p = plan[slot];
-            wire::DepositTransition t;
-            t.enabled = true;
-            t.before = wire_account(p.before); t.before_balances_hash = p.bal_hash; t.before_balance = wire_money(p.bal);
-            t.proof = wire_proof(s_proofs.data() + slot * A * 3, A);
-            t.account_index = p.idx; t.token_index = p.ti; t.balance_proof = wire_proof(forest.proofs.data() + p.e * T * 3, T);
-            sink->t.push_back(std::move(t));
-            sink->from.push_back(p.k);
-        }
-    }
+    BZK_TRY(list_root(ctx, 4, rev, &aux));
+    b.commit(aux, out->public3);
     return BZK_OK;
 }
 
-extern "C" {
-
-/* `mpn::withdraw::withdraw` (/root/reference/src/mpn/withdraw.rs:10-259): nonce, balances and the EdDSA signature over
- * Poseidon(fingerprint, nonce) are checked here (the hashes of a batch in two launches, the scalar multiplications on the
- * host).  Rows: raws1[slots][12] {enabled, token, amount, fee token, fee, fingerprint, pk.x, pk.y, nonce, sig.r.x, sig.r.y, sig.s},
- * raws2[slots][12+6T+3A] {account index, token index, fee token index, account before (4), token-tree hash, balance before (2),
- * its proof, fee balance before (2), its proof, account proof}, reveal[slots][7] {enabled, token, amount, fee token, fee,
- * fingerprint, calldata}. */
-int32_t bzk_mpn_withdraw_build(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_withdraw *wds, uint64_t n_wds, uint32_t log4_batch, bzk_fr *raws1,
-                               bzk_fr *raws2, bzk_fr *roots, bzk_fr *reveal, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted) {
-    return bzk::mpn_withdraw_build_impl(ctx, s, wds, n_wds, log4_batch, raws1, raws2, roots, reveal, accepted, public3, n_accepted, nullptr);
-}
-}  // extern "C"
-
-int32_t bzk::mpn_withdraw_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_withdraw *wds, uint64_t n_wds, uint32_t log4_batch, bzk_fr *raws1,
-                                     bzk_fr *raws2, bzk_fr *roots, bzk_fr *reveal, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted,
-                                     bzk::WithdrawSink *sink) {
-    if (!ctx || !s || (n_wds && !wds) || !raws1 || !raws2 || !roots || !reveal || !public3 || !n_accepted || log4_batch > 8) return BZK_ERR_BAD_ARG;
+// `mpn::withdraw::withdraw` (/root/reference/src/mpn/withdraw.rs:10-259): nonce, balances and the EdDSA signature over
+// Poseidon(fingerprint, nonce) are checked here (the hashes of a batch in two launches, the scalar multiplications on the host);
+// two steps per withdrawal (amount, then fee).  A withdrawal creates no account.
+int32_t bzk::mpn_withdraw_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_withdraw *wds, uint64_t n_wds, uint32_t log4_batch,
+                                     Built<wire::WithdrawTransition> *out) {
+    if (!ctx || !s || (n_wds && !wds) || !out || log4_batch > 8) return BZK_ERR_BAD_ARG;
     BZK_CUDA(ctx, cudaSetDevice(ctx->device));
-    const uint32_t A = s->A, T = s->T, w2 = 12 + 6 * T + 3 * A;
+    const uint32_t A = s->A, T = s->T;
     const uint64_t cap = 1ull << (2 * log4_batch);
-    const Fr prev_root = s->node(A, 0);
     // signature material of every candidate in two batched launches: msg = H(fingerprint, nonce), h = H(R.x, R.y, A.x, A.y, msg)
     std::vector<Point> addr(n_wds);
     std::vector<uint8_t> ok(n_wds, 0);
@@ -1209,154 +1092,112 @@ int32_t bzk::mpn_withdraw_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_m
         for (uint64_t k = 0; k < n_wds; k++)
             if (ok[k] && wds[k].check_calldata && (!canonical(wds[k].calldata) || !(cd[k] == fr_from_canon(&wds[k].calldata)))) ok[k] = 0;
     }
-    struct Plan { uint64_t k, idx; uint32_t ti, fi; Account before, mid, after; Money tok, fee_before; size_t e1, e2; Fr tok_hash; };
-    std::map<uint64_t, Account> mirror;
-    auto get = [&](uint64_t i) -> Account {
-        auto it = mirror.find(i);
-        if (it != mirror.end()) return it->second;
-        auto jt = s->accounts.find(i);
-        return jt == s->accounts.end() ? Account() : jt->second;
-    };
-    std::vector<Plan> plan;
-    for (uint64_t k = 0; k < n_wds; k++) {
-        if (accepted) accepted[k] = 0;
-        if (plan.size() == cap || !ok[k]) continue;
+    BatchCore b(s);
+    *out = Built<wire::WithdrawTransition>();
+    out->d.keys.assign(cap, null_key());
+    out->d.fingerprint.assign(cap, Fr::zero());
+    std::vector<Fr> cd_rows;
+    for (uint64_t k = 0; k < n_wds && out->t.size() < cap; k++) {
+        if (!ok[k]) continue;
         const bzk_mpn_withdraw &w = wds[k];
-        const auto key = std::make_pair(key_of(addr[k].x), key_of(addr[k].y));
         uint64_t idx = 0;
-        auto it = s->by_addr.find(key);
-        if (it != s->by_addr.end()) idx = it->second;
-        else {
-            auto jt = s->pending.find(key);
-            if (jt == s->pending.end()) continue;
-            idx = jt->second;
-        }
-        const Account before = get(idx);
+        if (!b.index_of(addr[k], &idx)) continue;
+        const Account before = b.get(idx);
         const Fr tok = fr_from_canon(&w.amount_token_id), ftok = fr_from_canon(&w.fee_token_id);
         const int ti = find_token_index(before, T, tok, false), fi = find_token_index(before, T, ftok, false);
         if (ti < 0 || fi < 0 || w.nonce != before.withdraw_nonce + 1) continue;
         if (before.tokens.at(ti).amount < w.amount) continue;
         Fr sig_s;
         memcpy(sig_s.l, &w.sig_s, 32);
-        if (!eddsa_verify_with_h(s, addr[k], Point{fr_from_canon(&w.sig_rx), fr_from_canon(&w.sig_ry)}, sig_s, hs[k])) continue;
-        Plan p{};
-        p.k = k; p.idx = idx; p.ti = (uint32_t)ti; p.fi = (uint32_t)fi; p.before = before; p.tok = before.tokens.at(ti);
-        p.mid = before;
-        p.mid.tokens[ti].amount -= w.amount;
-        if (p.mid.tokens.at(fi).amount < w.fee) continue;
-        p.fee_before = p.mid.tokens.at(fi);
-        p.after = p.mid;
-        p.after.tokens[fi].amount -= w.fee;
-        p.after.withdraw_nonce += 1;
-        mirror[idx] = p.after;
-        plan.push_back(std::move(p));
-        if (accepted) accepted[k] = 1;
+        const Point sig_r{fr_from_canon(&w.sig_rx), fr_from_canon(&w.sig_ry)};
+        if (!eddsa_verify_with_h(s, addr[k], sig_r, sig_s, hs[k])) continue;
+        Account mid = before;
+        mid.tokens[ti].amount -= w.amount;
+        if (mid.tokens.at(fi).amount < w.fee) continue;
+        Account after = mid;
+        after.tokens[fi].amount -= w.fee;
+        after.withdraw_nonce += 1;
+        b.step(idx, ti, mid);
+        b.step(idx, fi, after);
+        // `WithdrawTransition` (withdraw.rs:160-178)
+        wire::WithdrawTransition t;
+        t.enabled = true;
+        t.tx.mpn_address = wire::PubKey{addr[k].x, w.pk_odd != 0};
+        t.tx.nonce = w.nonce;
+        t.tx.sig.r = wire::PointW{sig_r.x, sig_r.y}; t.tx.sig.s = fr_from_canon(&w.sig_s);
+        t.tx.payment.amount = wire_money(Money{tok, w.amount}); t.tx.payment.fee = wire_money(Money{ftok, w.fee});
+        t.before = wire_account(before); t.before_token_balance = wire_money(before.tokens.at(ti)); t.before_fee_balance = wire_money(mid.tokens.at(fi));
+        t.account_index = idx; t.token_index = ti; t.fee_token_index = fi;
+        const size_t slot = out->t.size();
+        out->d.keys[slot] = wire::PointW{addr[k].x, addr[k].y};
+        out->d.fingerprint[slot] = fr_from_canon(&w.fingerprint);
+        for (const Fr &v : {addr[k].x, addr[k].y, fr_from_u64(w.nonce), sig_r.x, sig_r.y, t.tx.sig.s}) cd_rows.push_back(v);
+        out->t.push_back(std::move(t));
+        out->from.push_back(k);
     }
-    Forest forest;
-    forest.T = T;
-    std::vector<uint64_t> touched;
-    for (auto &p : plan)
-        if (forest.tree_of.emplace(p.idx, (uint32_t)forest.tree_of.size()).second) touched.push_back(p.idx);
-    for (uint64_t acc : touched) {
-        auto it = s->accounts.find(acc);
-        if (it != s->accounts.end())
-            for (auto &kv : it->second.tokens) forest.write(acc, kv.first, kv.second);
-    }
-    forest.n_init = forest.idx.size();
-    for (auto &p : plan) {
-        p.e1 = forest.write(p.idx, p.ti, p.mid.tokens[p.ti]);
-        p.e2 = forest.write(p.idx, p.fi, p.after.tokens[p.fi]);
-    }
-    BZK_TRY(forest.run(ctx, s->tdefaults));
-    std::vector<Fr> acct_rows, cd_rows;
-    auto push_acct = [&](const Account &a, const Fr &tok_root) {
-        acct_rows.push_back(fr_from_u64(a.tx_nonce)); acct_rows.push_back(fr_from_u64(a.withdraw_nonce));
-        acct_rows.push_back(a.ax); acct_rows.push_back(a.ay); acct_rows.push_back(tok_root);
-    };
-    for (auto &p : plan) {
-        p.tok_hash = forest.root(p.idx);
-        const Fr r1 = forest.applied(p.idx, p.e1), r2 = forest.applied(p.idx, p.e2);
-        push_acct(p.mid, r1); push_acct(p.after, r2);
-        const bzk_mpn_withdraw &w = wds[p.k];
-        cd_rows.push_back(addr[p.k].x); cd_rows.push_back(addr[p.k].y); cd_rows.push_back(fr_from_u64(w.nonce));
-        cd_rows.push_back(fr_from_canon(&w.sig_rx)); cd_rows.push_back(fr_from_canon(&w.sig_ry)); cd_rows.push_back(fr_from_canon(&w.sig_s));
-    }
-    std::vector<Fr> s_vals, s_proofs, cds;
-    BZK_TRY(hash_rows(ctx, 5, acct_rows, s_vals));
+    BZK_TRY(b.hash(ctx));
+    std::vector<Fr> cds;
     BZK_TRY(hash_rows(ctx, 6, cd_rows, cds));
-    std::vector<uint64_t> s_idx;
-    for (auto &p : plan) { s_idx.push_back(p.idx); s_idx.push_back(p.idx); }
-    const size_t ne = s_idx.size();
-    std::vector<Fr> init(ne * A * 3);
-    for (size_t e = 0; e < ne; e++) s->prove(s_idx[e], init.data() + e * A * 3);
-    BZK_TRY(tree_update_host(ctx, A, std::vector<uint32_t>(ne, 0u), s_idx, s_vals, init, s_proofs));
-    const Fr minus_one = Fr::one().neg();
-    Fr root = prev_root;
-    std::vector<Fr> rev_rows(cap * 7, Fr::zero());
-    for (uint64_t slot = 0; slot < cap; slot++) {
-        bzk_fr *r1 = raws1 + slot * 12, *r2 = raws2 + slot * w2, *rv = reveal + slot * 7;
-        memset(r1, 0, 12 * sizeof(bzk_fr)); memset(r2, 0, (size_t)w2 * sizeof(bzk_fr)); memset(rv, 0, 7 * sizeof(bzk_fr));
-        if (slot >= plan.size()) {
-            fr_to_canon(r1 + 7, minus_one);
-            continue;
-        }
-        const Plan &p = plan[slot];
-        const bzk_mpn_withdraw &w = wds[p.k];
-        fr_to_canon(roots + slot, root);
-        const uint64_t one = 1, nonce = w.nonce;
-        memcpy(r1 + 0, &one, 8); r1[1] = w.amount_token_id; memcpy(r1 + 2, &w.amount, 8); r1[3] = w.fee_token_id; memcpy(r1 + 4, &w.fee, 8);
-        r1[5] = w.fingerprint; fr_to_canon(r1 + 6, addr[p.k].x); fr_to_canon(r1 + 7, addr[p.k].y); memcpy(r1 + 8, &nonce, 8);
-        r1[9] = w.sig_rx; r1[10] = w.sig_ry; r1[11] = w.sig_s;
-        size_t q = 0;
-        auto put_fr = [&](const Fr &v) { fr_to_canon(r2 + (q++), v); };
-        auto put_u = [&](uint64_t v) { memcpy(r2 + (q++), &v, 8); };
-        put_u(p.idx); put_u(p.ti); put_u(p.fi); put_u(p.before.tx_nonce); put_u(p.before.withdraw_nonce); put_fr(p.before.ax); put_fr(p.before.ay);
-        put_fr(p.tok_hash); put_fr(p.tok.token_id); put_u(p.tok.amount);
-        for (uint32_t i = 0; i < T * 3; i++) put_fr(forest.proofs[p.e1 * T * 3 + i]);
-        put_fr(p.fee_before.token_id); put_u(p.fee_before.amount);
-        for (uint32_t i = 0; i < T * 3; i++) put_fr(forest.proofs[p.e2 * T * 3 + i]);
-        for (uint32_t i = 0; i < A * 3; i++) put_fr(s_proofs[(2 * slot) * A * 3 + i]);
-        if (q != w2) return BZK_ERR_BAD_ARG;
-        memcpy(rv + 0, &one, 8); rv[1] = w.amount_token_id; memcpy(rv + 2, &w.amount, 8); rv[3] = w.fee_token_id; memcpy(rv + 4, &w.fee, 8);
-        rv[5] = w.fingerprint; fr_to_canon(rv + 6, cds[slot]);
-        Fr *rr = rev_rows.data() + slot * 7;
-        rr[0] = Fr::one(); rr[1] = fr_from_canon(&w.amount_token_id); rr[2] = fr_from_u64(w.amount); rr[3] = fr_from_canon(&w.fee_token_id);
-        rr[4] = fr_from_u64(w.fee); rr[5] = fr_from_canon(&w.fingerprint); rr[6] = cds[slot];
-        root = s_vals[(size_t)A * ne + 2 * slot + 1];
+    cds.resize(cap, Fr::zero());
+    out->d.calldata = cds;
+    for (size_t k = 0; k < out->t.size(); k++) {
+        wire::WithdrawTransition &t = out->t[k];
+        t.before_token_hash = b.tok_before(2 * k); t.token_balance_proof = b.tok_proof(2 * k); t.fee_balance_proof = b.tok_proof(2 * k + 1);
+        t.proof = b.state_proof(2 * k);
     }
-    for (uint64_t slot = plan.size(); slot < cap; slot++) fr_to_canon(roots + slot, root);
-    for (size_t e = 0; e < ne; e++) {
-        uint64_t node = s_idx[e];
-        for (uint32_t l = 0; l <= A; l++) { s->put(l, node, s_vals[(size_t)l * ne + e]); node >>= 2; }
-    }
-    for (uint64_t i : touched) {
-        auto it = s->accounts.find(i);
-        if (it != s->accounts.end()) s->state_size -= leaf_count(it->second);
-        s->state_size += leaf_count(mirror[i]);
-        s->accounts[i] = mirror[i];
-    }
+    out->d.roots = b.slot_roots(cap, 2);
+    std::vector<wire::WithdrawTransition> slots;
+    padded(out->t, log4_batch, null_withdraw(A, T), slots);
+    std::vector<Fr> rev(cap * 7);
+    for (uint64_t k = 0; k < cap; k++) withdraw_reveal(slots[k], out->d, k, rev.data() + k * 7);
     Fr aux;
-    BZK_TRY(list_root(ctx, 7, rev_rows, &aux));
-    fr_to_canon(public3 + 0, prev_root);
-    fr_to_canon(public3 + 1, aux);
-    fr_to_canon(public3 + 2, root);
-    *n_accepted = plan.size();
-    if (sink) {   // `WithdrawTransition` of every accepted withdrawal (/root/reference/src/mpn/withdraw.rs:160-178)
-        sink->t.clear(); sink->from.clear();
-        for (size_t slot = 0; slot < plan.size(); slot++) {
-            const Plan &p = plan[slot];
-            wire::WithdrawTransition t;
-            t.enabled = true;
-            t.before = wire_account(p.before); t.before_token_balance = wire_money(p.tok); t.before_fee_balance = wire_money(p.fee_before);
-            t.proof = wire_proof(s_proofs.data() + (2 * slot) * A * 3, A);
-            t.account_index = p.idx; t.token_index = p.ti; t.token_balance_proof = wire_proof(forest.proofs.data() + p.e1 * T * 3, T);
-            t.before_token_hash = p.tok_hash; t.fee_token_index = p.fi; t.fee_balance_proof = wire_proof(forest.proofs.data() + p.e2 * T * 3, T);
-            sink->t.push_back(std::move(t));
-            sink->from.push_back(p.k);
-        }
-    }
+    BZK_TRY(list_root(ctx, 7, rev, &aux));
+    b.commit(aux, out->public3);
     return BZK_OK;
 }
+
+extern "C" {
+
+/* The builders' C ABI (include/bzk.h): the rows of the padded batch by the circuit's writer (csrc/mpn_wire.cu).  The ledger
+ * advances (build on a clone, see bzk_mpn_state_clone). */
+int32_t bzk_mpn_update_build(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_tx *txs, uint64_t n_txs, uint32_t log4_batch,
+                             const bzk_fr *fee_token_canon, bzk_fr *raws, bzk_fr *ext, uint8_t *accepted, bzk_fr public3[3],
+                             uint64_t *n_accepted) {
+    if (!raws || !ext || !public3 || !n_accepted) return BZK_ERR_BAD_ARG;
+    Built<wire::UpdateTransition> bt;
+    BZK_TRY(mpn_update_build_impl(ctx, s, txs, n_txs, log4_batch, fee_token_canon, &bt));
+    std::vector<wire::UpdateTransition> slots;
+    padded(bt.t, log4_batch, null_update(s->A, s->T), slots);
+    BZK_TRY(write_update_rows(slots, bt.d, s->A, s->T, fr_from_canon(fee_token_canon), raws, ext));
+    report(bt, n_txs, accepted, public3, n_accepted);
+    return BZK_OK;
+}
+
+int32_t bzk_mpn_deposit_build(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_deposit *deps, uint64_t n_deps, uint32_t log4_batch, bzk_fr *raws1,
+                              bzk_fr *raws2, bzk_fr *roots, bzk_fr *reveal, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted) {
+    if (!raws1 || !raws2 || !roots || !reveal || !public3 || !n_accepted) return BZK_ERR_BAD_ARG;
+    Built<wire::DepositTransition> bt;
+    BZK_TRY(mpn_deposit_build_impl(ctx, s, deps, n_deps, log4_batch, &bt));
+    std::vector<wire::DepositTransition> slots;
+    padded(bt.t, log4_batch, null_deposit(s->A, s->T), slots);
+    BZK_TRY(write_deposit_rows(slots, bt.d, s->A, s->T, raws1, raws2, roots, reveal));
+    report(bt, n_deps, accepted, public3, n_accepted);
+    return BZK_OK;
+}
+
+int32_t bzk_mpn_withdraw_build(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_withdraw *wds, uint64_t n_wds, uint32_t log4_batch, bzk_fr *raws1,
+                               bzk_fr *raws2, bzk_fr *roots, bzk_fr *reveal, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted) {
+    if (!raws1 || !raws2 || !roots || !reveal || !public3 || !n_accepted) return BZK_ERR_BAD_ARG;
+    Built<wire::WithdrawTransition> bt;
+    BZK_TRY(mpn_withdraw_build_impl(ctx, s, wds, n_wds, log4_batch, &bt));
+    std::vector<wire::WithdrawTransition> slots;
+    padded(bt.t, log4_batch, null_withdraw(s->A, s->T), slots);
+    BZK_TRY(write_withdraw_rows(slots, bt.d, s->A, s->T, raws1, raws2, roots, reveal));
+    report(bt, n_wds, accepted, public3, n_accepted);
+    return BZK_OK;
+}
+
+}  // extern "C"
 
 // ---------------------------------------------------------------------------------------------
 // witness of a whole deposit / withdraw batch from the builder's rows: what `{Deposit,Withdraw}Circuit::synthesize`
@@ -1397,9 +1238,6 @@ extern "C" int32_t bzk_mpn_dw_witness(bzk_ctx *ctx, const bzk_witness_program *p
     BZK_TRY(bzk_witness_run_dev(ctx, phase2, raws2, ext.data(), n_slots, z_aux + 5 + n_slots * n1 + nr));
     return BZK_OK;
 }
-
-extern "C" {
-}  // extern "C"
 
 // ---------------------------------------------------------------------------------------------
 // witness of a whole update batch from the builder's rows: what `UpdateCircuit::synthesize` assigns

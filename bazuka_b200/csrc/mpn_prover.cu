@@ -125,15 +125,15 @@ int32_t bzk_mpn_prover_prove_work(bzk_ctx *ctx, bzk_mpn_prover *p, const uint8_t
     height.l[0] = info.height;
     Fr *z_in = (Fr *)p->d_z, *z_aux = z_in + p->shape[0];
     if (p->kind == 0) {
-        const uint32_t n_raw = 32 + 9 * p->T + 6 * p->A;
+        const uint32_t n_raw = update_raw_width(p->A, p->T);
         std::vector<bzk_fr> raws(n * n_raw), ext(n * 2);
         BZK_TRY(bzk_mpn_work_update_rows_ctx(ctx, work.get(), &p->jj_d, &p->fee_token, raws.data(), ext.data()));
         const bzk_fr prologue[6] = {commitment, height, info.state, p->fee_token, info.aux_data, info.next_state};
         BZK_TRY(bzk_mpn_update_witness(ctx, p->prog[0], p->prog[1], n, p->T, p->shape[7], p->shape[10], raws.data(), ext.data(), n_raw, prologue, z_in,
                                        z_aux));
     } else {
-        const uint32_t w1 = p->kind == 1 ? 5 : 12, w2 = p->kind == 1 ? 9 + 3 * p->T + 3 * p->A : 12 + 6 * p->T + 3 * p->A, wr = p->kind == 1 ? 4 : 7;
-        std::vector<bzk_fr> raws1(n * w1), raws2(n * w2), roots(n), reveal(n * wr);
+        const DwWidths w = p->kind == 1 ? deposit_widths(p->A, p->T) : withdraw_widths(p->A, p->T);
+        std::vector<bzk_fr> raws1(n * w.raw1), raws2(n * w.raw2), roots(n), reveal(n * w.reveal);
         BZK_TRY(bzk_mpn_work_dw_rows_ctx(ctx, work.get(), &p->jj_d, raws1.data(), raws2.data(), roots.data(), reveal.data()));
         const bzk_fr public5[5] = {commitment, height, info.state, info.aux_data, info.next_state};
         BZK_TRY(bzk_mpn_dw_witness(ctx, p->prog[0], p->prog[1], p->prog[2], n, raws1.data(), raws2.data(), roots.data(), p->ext_src.data(),

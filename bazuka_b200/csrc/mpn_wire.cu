@@ -112,7 +112,7 @@ void dec_proof(Reader &r, Proof &p) {
     for (Fr &v : p) v = r.fr();
 }
 void enc_account(Writer &w, const Account &a) {
-    w.u32(a.tx_nonce); w.u32(a.withdraw_nonce); enc_point(w, a.address);
+    w.u32((uint32_t)a.tx_nonce); w.u32((uint32_t)a.withdraw_nonce); enc_point(w, a.address);
     w.u64(a.tokens.size());
     for (auto &kv : a.tokens) { w.u64(kv.first); enc_money(w, kv.second); }
 }
@@ -128,7 +128,7 @@ void dec_account(Reader &r, Account &a) {
     }
 }
 void enc_mpn_tx(Writer &w, const MpnTx &t) {
-    w.u32(t.nonce); enc_pubkey(w, t.src); enc_pubkey(w, t.dst); enc_money(w, t.amount); enc_money(w, t.fee); enc_sig(w, t.sig);
+    w.u32((uint32_t)t.nonce); enc_pubkey(w, t.src); enc_pubkey(w, t.dst); enc_money(w, t.amount); enc_money(w, t.fee); enc_sig(w, t.sig);
 }
 void dec_mpn_tx(Reader &r, MpnTx &t) {
     t.nonce = r.u32(); dec_pubkey(r, t.src); dec_pubkey(r, t.dst); dec_money(r, t.amount); dec_money(r, t.fee); dec_sig(r, t.sig);
@@ -308,7 +308,6 @@ using namespace bzk::wire;
 struct bzk_mpn_work { Work w; };
 
 namespace {
-inline void canon_out(bzk_fr *out, const Fr &mont) { Fr c = mont.from_mont(); memcpy(out, c.l, 32); }
 inline void put_u(bzk_fr *out, uint64_t v) { memset(out, 0, 32); memcpy(out, &v, 8); }
 
 // batched Poseidon, in[n][arity] -> out[n] (Montgomery images): the host hasher, or a context's batched launch
@@ -324,11 +323,14 @@ struct RootJob {   // one enabled transition: its account before, the balances h
 struct RowCtx {
     HashBatch hash;
     const bzk_fr *jj_d;
-    // PublicKey::decompress -> canonical affine point
-    int32_t decompress(const PubKey &k, bzk_fr out[2]) const {
-        bzk_fr x;
-        canon_out(&x, k.x);
-        return bzk_jubjub_decompress(jj_d, &x, k.odd ? 1 : 0, out);
+    // PublicKey::decompress -> affine point
+    int32_t decompress(const PubKey &k, PointW *out) const {
+        bzk_fr x, xy[2];
+        fr_to_canon(&x, k.x);
+        BZK_TRY(bzk_jubjub_decompress(jj_d, &x, k.odd ? 1 : 0, xy));
+        memcpy(out->x.l, xy + 0, 32); memcpy(out->y.l, xy + 1, 32);
+        out->x = out->x.to_mont(); out->y = out->y.to_mont();
+        return BZK_OK;
     }
     // The state root each job's transition was built against: leaf H(tx_nonce, withdraw_nonce, addr, balances hash), then
     // `calc_root_poseidon4` (/root/reference/src/zk/groth16/gadgets/merkle/mod.rs:53-65) under the transition's own proof —
@@ -342,7 +344,7 @@ struct RowCtx {
         for (size_t j = 0; j < n; j++) {
             const Account &a = *jobs[j].account;
             Fr *row = in.data() + j * 5;
-            row[0] = Fr::from_u32(a.tx_nonce); row[1] = Fr::from_u32(a.withdraw_nonce); row[2] = a.address.x; row[3] = a.address.y;
+            row[0] = fr_from_u64(a.tx_nonce); row[1] = fr_from_u64(a.withdraw_nonce); row[2] = a.address.x; row[3] = a.address.y;
             row[4] = jobs[j].balances_hash;
         }
         BZK_TRY(hash(5, in.data(), n, cur.data()));
@@ -377,34 +379,6 @@ void slot_roots(const std::vector<T> &ts, const Fr &state, const Fr &next_state,
 }
 bool proofs_shaped(const Proof &p, uint32_t levels) { return p.size() == (size_t)levels * 3; }
 
-// `{Update,Deposit,Withdraw}Transition::null` (/root/reference/src/mpn/mod.rs:440-537): what the prover pads a batch with — a work
-// carries only the transitions the builder made, the circuit always has 4^B slots
-UpdateTransition null_update(uint32_t A, uint32_t T) {
-    UpdateTransition t;
-    t.src_proof.assign(3 * A, Fr::zero()); t.dst_proof.assign(3 * A, Fr::zero());
-    t.src_balance_proof.assign(3 * T, Fr::zero()); t.src_fee_balance_proof.assign(3 * T, Fr::zero()); t.dst_balance_proof.assign(3 * T, Fr::zero());
-    return t;
-}
-DepositTransition null_deposit(uint32_t A, uint32_t T) {
-    DepositTransition t;
-    t.proof.assign(3 * A, Fr::zero()); t.balance_proof.assign(3 * T, Fr::zero());
-    return t;
-}
-WithdrawTransition null_withdraw(uint32_t A, uint32_t T) {
-    WithdrawTransition t;
-    t.proof.assign(3 * A, Fr::zero()); t.token_balance_proof.assign(3 * T, Fr::zero()); t.fee_balance_proof.assign(3 * T, Fr::zero());
-    return t;
-}
-// the batch of a work padded to its 4^B slots; false when the work holds more transitions than its config allows
-template <class T>
-bool padded(const std::vector<T> &ts, uint32_t log4_batch, const T &null, std::vector<T> &out) {
-    if (log4_batch > 8) return false;
-    const size_t slots = (size_t)1 << (2 * log4_batch);
-    if (ts.size() > slots) return false;
-    out = ts;
-    out.resize(slots, null);
-    return true;
-}
 }  // namespace
 
 extern "C" {
@@ -442,8 +416,8 @@ int32_t bzk_mpn_work_get_info(const bzk_mpn_work *w, bzk_mpn_work_info *out) {
     memset(out, 0, sizeof *out);
     out->kind = k.kind; out->log4_tree = k.config.log4_tree; out->log4_token = k.config.log4_token; out->log4_batch = k.log4_batch();
     out->n_transitions = k.n_transitions(); out->height = k.height; out->reward = k.reward; out->new_root_size = k.new_root_size;
-    canon_out(&out->state, k.state); canon_out(&out->aux_data, k.aux_data); canon_out(&out->next_state, k.next_state);
-    canon_out(&out->new_root_hash, k.new_root_hash);
+    fr_to_canon(&out->state, k.state); fr_to_canon(&out->aux_data, k.aux_data); fr_to_canon(&out->next_state, k.next_state);
+    fr_to_canon(&out->new_root_hash, k.new_root_hash);
     return BZK_OK;
 }
 
@@ -456,7 +430,7 @@ int32_t bzk_mpn_work_vk(const bzk_mpn_work *w, const uint8_t **vk, size_t *len) 
 
 int32_t bzk_mpn_commitment(const uint8_t prover[32], uint64_t reward, bzk_fr *out) {
     if (!prover || !out) return BZK_ERR_BAD_ARG;
-    canon_out(out, commitment(prover, reward));
+    fr_to_canon(out, commitment(prover, reward));
     return BZK_OK;
 }
 
@@ -470,7 +444,7 @@ int32_t bzk_sha3_256(const uint8_t *data, size_t len, uint8_t out[32]) {
  * images as bzk_groth16_verify_bytes takes them */
 int32_t bzk_mpn_work_public_inputs(const bzk_mpn_work *w, const uint8_t prover[32], bzk_fr out[5]) {
     if (!w || !prover || !out) return BZK_ERR_BAD_ARG;
-    const Fr v[5] = {commitment(prover, w->w.reward), fr_of_u64(w->w.height), w->w.state, w->w.aux_data, w->w.next_state};
+    const Fr v[5] = {commitment(prover, w->w.reward), fr_from_u64(w->w.height), w->w.state, w->w.aux_data, w->w.next_state};
     memcpy(out, v, sizeof v);
     return BZK_OK;
 }
@@ -486,150 +460,209 @@ int32_t bzk_mpn_work_verify(const bzk_mpn_work *w, const uint8_t prover[32], con
 
 }  // extern "C"
 
-namespace {
+// ------------------------------------------------------------------------------------------------ circuit rows
+namespace bzk {
 
-// An update work's transitions as the rows bzk_mpn_update_witness consumes (the order of UpdateCircuit's allocations,
-// `bazuka_b200/mpn/witness_program.py::raw_values`): raws[4^B][32 + 9T + 6A], ext[4^B][2] = {fee token, state root entering the
-// slot} — the root is not on the wire: recomputed from the transition's own account, proof and index.  A work carries only the
-// transitions its builder made; the slots after them are padded as `UpdateTransition::null`.  Canonical scalars.
-int32_t update_rows(const Work &k, const RowCtx &rc, const bzk_fr *fee_token, bzk_fr *raws, bzk_fr *ext) {
-    const uint32_t A = k.config.log4_tree, T = k.config.log4_token, n_raw = 32 + 9 * T + 6 * A;
-    std::vector<UpdateTransition> updates;
-    if (!padded(k.updates, k.config.log4_update_batch, null_update(A, T), updates)) return BZK_ERR_BAD_ARG;
-    std::vector<RootJob> jobs;
-    for (const UpdateTransition &t : updates) {
-        if (!proofs_shaped(t.src_proof, A) || !proofs_shaped(t.dst_proof, A) || !proofs_shaped(t.src_balance_proof, T) ||
-            !proofs_shaped(t.src_fee_balance_proof, T) || !proofs_shaped(t.dst_balance_proof, T))
-            return BZK_ERR_BAD_ARG;
-        if (t.enabled) jobs.push_back(RootJob{&t.src_before, t.src_before_balances_hash, t.src_index, &t.src_proof});
-    }
-    std::vector<Fr> enabled_roots, roots;
-    BZK_TRY(rc.entering_roots(jobs, A, enabled_roots));
-    slot_roots(updates, k.state, k.next_state, enabled_roots, roots);
-    for (size_t s = 0; s < updates.size(); s++) {
-        const UpdateTransition &t = updates[s];
-        bzk_fr *row = raws + s * n_raw;
-        size_t w = 0;
-        auto fr = [&](const Fr &v) { canon_out(row + (w++), v); };
-        auto u = [&](uint64_t v) { put_u(row + (w++), v); };
-        auto proof = [&](const Proof &p) { for (const Fr &v : p) fr(v); };
-        bzk_fr dst_pk[2];
-        BZK_TRY(rc.decompress(t.tx.dst, dst_pk));
-        u(t.enabled ? 1 : 0); u(t.src_token_index); u(t.src_fee_token_index); u(t.dst_token_index);
-        u(t.src_before.tx_nonce); u(t.src_before.withdraw_nonce); fr(t.src_before.address.x); fr(t.src_before.address.y);
-        fr(t.src_before_balances_hash); fr(t.dst_before_balances_hash);
-        fr(t.src_before_balance.token.scalar()); u(t.src_before_balance.amount);
-        fr(t.src_before_fee_balance.token.scalar()); u(t.src_before_fee_balance.amount);
-        proof(t.src_balance_proof);
-        u(t.tx.amount.amount); u(t.tx.fee.amount);
-        proof(t.src_fee_balance_proof);
-        u(t.tx.nonce); u(t.src_index); fr(t.tx.amount.token.scalar()); fr(t.tx.fee.token.scalar());
-        fr(t.dst_before_balance.token.scalar()); u(t.dst_before_balance.amount);
-        proof(t.dst_balance_proof);
-        proof(t.src_proof);
-        row[w++] = dst_pk[0]; row[w++] = dst_pk[1]; u(t.dst_index);
-        u(t.dst_before.tx_nonce); u(t.dst_before.withdraw_nonce); fr(t.dst_before.address.x); fr(t.dst_before.address.y);
-        proof(t.dst_proof);
-        fr(t.tx.sig.r.x); fr(t.tx.sig.r.y); fr(t.tx.sig.s);
-        if (w != n_raw) return BZK_ERR_BAD_ARG;
-        ext[2 * s] = *fee_token;
-        canon_out(ext + 2 * s + 1, roots[s]);
+UpdateTransition null_update(uint32_t A, uint32_t T) {
+    UpdateTransition t;
+    t.src_proof.assign(3 * A, Fr::zero()); t.dst_proof.assign(3 * A, Fr::zero());
+    t.src_balance_proof.assign(3 * T, Fr::zero()); t.src_fee_balance_proof.assign(3 * T, Fr::zero()); t.dst_balance_proof.assign(3 * T, Fr::zero());
+    return t;
+}
+DepositTransition null_deposit(uint32_t A, uint32_t T) {
+    DepositTransition t;
+    t.proof.assign(3 * A, Fr::zero()); t.balance_proof.assign(3 * T, Fr::zero());
+    return t;
+}
+WithdrawTransition null_withdraw(uint32_t A, uint32_t T) {
+    WithdrawTransition t;
+    t.proof.assign(3 * A, Fr::zero()); t.token_balance_proof.assign(3 * T, Fr::zero()); t.fee_balance_proof.assign(3 * T, Fr::zero());
+    return t;
+}
+
+void deposit_reveal(const DepositTransition &t, const SlotData &d, size_t slot, Fr out[4]) {
+    out[0] = t.enabled ? Fr::one() : Fr::zero(); out[1] = t.tx.payment.amount.token.scalar(); out[2] = fr_from_u64(t.tx.payment.amount.amount);
+    out[3] = d.pk_hash[slot];   // deposit_circuit.rs: the calldata of a deposit is the hash of its MPN key
+}
+void withdraw_reveal(const WithdrawTransition &t, const SlotData &d, size_t slot, Fr out[7]) {
+    const ContractWithdraw &p = t.tx.payment;
+    out[0] = t.enabled ? Fr::one() : Fr::zero(); out[1] = p.amount.token.scalar(); out[2] = fr_from_u64(p.amount.amount);
+    out[3] = p.fee.token.scalar(); out[4] = fr_from_u64(p.fee.amount); out[5] = d.fingerprint[slot]; out[6] = d.calldata[slot];
+}
+
+namespace {
+// appends scalars to one row of a circuit's inputs, canonical
+struct RowWriter {
+    bzk_fr *row;
+    size_t w = 0;
+    void fr(const Fr &v) { fr_to_canon(row + (w++), v); }
+    void u(uint64_t v) { put_u(row + (w++), v); }
+    void proof(const Proof &p) { for (const Fr &v : p) fr(v); }
+    void account(const Account &a) { u(a.tx_nonce); u(a.withdraw_nonce); fr(a.address.x); fr(a.address.y); }
+    void money(const Money &m) { fr(m.token.scalar()); u(m.amount); }
+};
+}  // namespace
+
+// the order of UpdateCircuit's allocations (`bazuka_b200/mpn/witness_program.py::raw_values`)
+int32_t write_update_rows(const std::vector<UpdateTransition> &ts, const SlotData &d, uint32_t A, uint32_t T, const Fr &fee_token, bzk_fr *raws,
+                          bzk_fr *ext) {
+    const uint32_t n_raw = update_raw_width(A, T);
+    for (size_t s = 0; s < ts.size(); s++) {
+        const UpdateTransition &t = ts[s];
+        RowWriter r{raws + s * n_raw};
+        r.u(t.enabled ? 1 : 0); r.u(t.src_token_index); r.u(t.src_fee_token_index); r.u(t.dst_token_index);
+        r.account(t.src_before);
+        r.fr(t.src_before_balances_hash); r.fr(t.dst_before_balances_hash);
+        r.money(t.src_before_balance); r.money(t.src_before_fee_balance);
+        r.proof(t.src_balance_proof);
+        r.u(t.tx.amount.amount); r.u(t.tx.fee.amount);
+        r.proof(t.src_fee_balance_proof);
+        r.u(t.tx.nonce); r.u(t.src_index); r.fr(t.tx.amount.token.scalar()); r.fr(t.tx.fee.token.scalar());
+        r.money(t.dst_before_balance);
+        r.proof(t.dst_balance_proof);
+        r.proof(t.src_proof);
+        r.fr(d.keys[s].x); r.fr(d.keys[s].y); r.u(t.dst_index);
+        r.account(t.dst_before);
+        r.proof(t.dst_proof);
+        r.fr(t.tx.sig.r.x); r.fr(t.tx.sig.r.y); r.fr(t.tx.sig.s);
+        if (r.w != n_raw) return BZK_ERR_BAD_ARG;
+        fr_to_canon(ext + 2 * s, fee_token);
+        fr_to_canon(ext + 2 * s + 1, d.roots[s]);
     }
     return BZK_OK;
 }
 
-// A deposit / withdraw work's transitions as the rows bzk_mpn_dw_witness consumes (layouts: bzk_mpn_deposit_build /
-// bzk_mpn_withdraw_build): raws1, raws2, the entering roots and the revealed rows, canonical scalars.  The calldata hash of
-// every enabled slot's revealed row in ONE batched hash.
+// raws1 {enabled, token, amount, pk.x, pk.y}; raws2 {account index, token index, account before (4), balances hash, balance
+// before (2), balance proof, account proof}
+int32_t write_deposit_rows(const std::vector<DepositTransition> &ts, const SlotData &d, uint32_t A, uint32_t T, bzk_fr *raws1, bzk_fr *raws2,
+                           bzk_fr *roots, bzk_fr *reveal) {
+    const DwWidths wd = deposit_widths(A, T);
+    for (size_t s = 0; s < ts.size(); s++) {
+        const DepositTransition &t = ts[s];
+        RowWriter r1{raws1 + s * wd.raw1}, r2{raws2 + s * wd.raw2};
+        r1.u(t.enabled ? 1 : 0); r1.money(t.tx.payment.amount); r1.fr(d.keys[s].x); r1.fr(d.keys[s].y);
+        r2.u(t.account_index); r2.u(t.token_index); r2.account(t.before);
+        r2.fr(t.before_balances_hash); r2.money(t.before_balance);
+        r2.proof(t.balance_proof);
+        r2.proof(t.proof);
+        if (r2.w != wd.raw2) return BZK_ERR_BAD_ARG;
+        Fr rv[4];
+        deposit_reveal(t, d, s, rv);
+        for (int i = 0; i < 4; i++) fr_to_canon(reveal + s * wd.reveal + i, rv[i]);
+        fr_to_canon(roots + s, d.roots[s]);
+    }
+    return BZK_OK;
+}
+
+// raws1 {enabled, token, amount, fee token, fee, fingerprint, pk.x, pk.y, nonce, sig.r.x, sig.r.y, sig.s}; raws2 {account index,
+// token index, fee token index, account before (4), token-tree hash, balance before (2), its proof, fee balance before (2), its
+// proof, account proof}
+int32_t write_withdraw_rows(const std::vector<WithdrawTransition> &ts, const SlotData &d, uint32_t A, uint32_t T, bzk_fr *raws1, bzk_fr *raws2,
+                            bzk_fr *roots, bzk_fr *reveal) {
+    const DwWidths wd = withdraw_widths(A, T);
+    for (size_t s = 0; s < ts.size(); s++) {
+        const WithdrawTransition &t = ts[s];
+        const ContractWithdraw &p = t.tx.payment;
+        RowWriter r1{raws1 + s * wd.raw1}, r2{raws2 + s * wd.raw2};
+        r1.u(t.enabled ? 1 : 0); r1.money(p.amount); r1.money(p.fee); r1.fr(d.fingerprint[s]);
+        r1.fr(d.keys[s].x); r1.fr(d.keys[s].y); r1.u(t.tx.nonce);
+        r1.fr(t.tx.sig.r.x); r1.fr(t.tx.sig.r.y); r1.fr(t.tx.sig.s);
+        r2.u(t.account_index); r2.u(t.token_index); r2.u(t.fee_token_index); r2.account(t.before);
+        r2.fr(t.before_token_hash); r2.money(t.before_token_balance);
+        r2.proof(t.token_balance_proof);
+        r2.money(t.before_fee_balance);
+        r2.proof(t.fee_balance_proof);
+        r2.proof(t.proof);
+        if (r2.w != wd.raw2) return BZK_ERR_BAD_ARG;
+        Fr rv[7];
+        withdraw_reveal(t, d, s, rv);
+        for (int i = 0; i < 7; i++) fr_to_canon(reveal + s * wd.reveal + i, rv[i]);
+        fr_to_canon(roots + s, d.roots[s]);
+    }
+    return BZK_OK;
+}
+
+}  // namespace bzk
+
+namespace {
+
+// An update work's rows (write_update_rows).  The entering roots are not on the wire: recomputed from each transition's own
+// account, proof and index.
+int32_t update_rows(const Work &k, const RowCtx &rc, const bzk_fr *fee_token, bzk_fr *raws, bzk_fr *ext) {
+    const uint32_t A = k.config.log4_tree, T = k.config.log4_token;
+    std::vector<UpdateTransition> updates;
+    if (!padded(k.updates, k.config.log4_update_batch, null_update(A, T), updates)) return BZK_ERR_BAD_ARG;
+    SlotData d;
+    d.keys.resize(updates.size());
+    std::vector<RootJob> jobs;
+    for (size_t s = 0; s < updates.size(); s++) {
+        const UpdateTransition &t = updates[s];
+        if (!proofs_shaped(t.src_proof, A) || !proofs_shaped(t.dst_proof, A) || !proofs_shaped(t.src_balance_proof, T) ||
+            !proofs_shaped(t.src_fee_balance_proof, T) || !proofs_shaped(t.dst_balance_proof, T))
+            return BZK_ERR_BAD_ARG;
+        BZK_TRY(rc.decompress(t.tx.dst, &d.keys[s]));
+        if (t.enabled) jobs.push_back(RootJob{&t.src_before, t.src_before_balances_hash, t.src_index, &t.src_proof});
+    }
+    std::vector<Fr> enabled_roots;
+    BZK_TRY(rc.entering_roots(jobs, A, enabled_roots));
+    slot_roots(updates, k.state, k.next_state, enabled_roots, d.roots);
+    Fr fee;
+    memcpy(fee.l, fee_token, 32);
+    return write_update_rows(updates, d, A, T, fee.to_mont(), raws, ext);
+}
+
+// A deposit / withdraw work's rows (write_deposit_rows / write_withdraw_rows).  The calldata hash of every enabled slot's
+// revealed row in ONE batched hash.
 int32_t dw_rows(const Work &k, const RowCtx &rc, bzk_fr *raws1, bzk_fr *raws2, bzk_fr *roots_out, bzk_fr *reveal) {
     const uint32_t A = k.config.log4_tree, T = k.config.log4_token;
-    std::vector<Fr> enabled_roots, roots, cd_in, cd;
+    std::vector<Fr> enabled_roots, cd_in, cd;
     std::vector<RootJob> jobs;
-    auto mont_of = [](const bzk_fr &c) { Fr v; memcpy(v.l, &c, 32); return v.to_mont(); };
+    std::vector<size_t> enabled;
+    SlotData d;
+    auto finish = [&](uint32_t arity, std::vector<Fr> &per_slot) -> int32_t {   // the calldata hashes, spread over the slots
+        BZK_TRY(rc.entering_roots(jobs, A, enabled_roots));
+        cd.assign(jobs.size(), Fr::zero());
+        if (!jobs.empty()) BZK_TRY(rc.hash(arity, cd_in.data(), jobs.size(), cd.data()));
+        per_slot.assign(d.keys.size(), Fr::zero());
+        for (size_t e = 0; e < enabled.size(); e++) per_slot[enabled[e]] = cd[e];
+        return BZK_OK;
+    };
     if (k.kind == KIND_DEPOSIT) {
-        const uint32_t w2 = 9 + 3 * T + 3 * A;
         std::vector<DepositTransition> deposits;
         if (!padded(k.deposits, k.config.log4_deposit_batch, null_deposit(A, T), deposits)) return BZK_ERR_BAD_ARG;
-        std::vector<bzk_fr> pks(deposits.size() * 2);
+        d.keys.resize(deposits.size());
         for (size_t s = 0; s < deposits.size(); s++) {
             const DepositTransition &t = deposits[s];
             if (!proofs_shaped(t.proof, A) || !proofs_shaped(t.balance_proof, T)) return BZK_ERR_BAD_ARG;
-            BZK_TRY(rc.decompress(t.tx.mpn_address, pks.data() + 2 * s));
+            BZK_TRY(rc.decompress(t.tx.mpn_address, &d.keys[s]));
             if (!t.enabled) continue;
             jobs.push_back(RootJob{&t.before, t.before_balances_hash, t.account_index, &t.proof});
-            cd_in.push_back(mont_of(pks[2 * s])); cd_in.push_back(mont_of(pks[2 * s + 1]));
+            enabled.push_back(s);
+            cd_in.push_back(d.keys[s].x); cd_in.push_back(d.keys[s].y);
         }
-        BZK_TRY(rc.entering_roots(jobs, A, enabled_roots));
-        slot_roots(deposits, k.state, k.next_state, enabled_roots, roots);
-        cd.assign(jobs.size(), Fr::zero());
-        if (!jobs.empty()) BZK_TRY(rc.hash(2, cd_in.data(), jobs.size(), cd.data()));
-        size_t e = 0;
-        for (size_t s = 0; s < deposits.size(); s++) {
-            const DepositTransition &t = deposits[s];
-            const bzk_fr *pk = pks.data() + 2 * s;
-            bzk_fr *r1 = raws1 + s * 5, *r2 = raws2 + s * w2, *rv = reveal + s * 4;
-            put_u(r1 + 0, t.enabled ? 1 : 0); canon_out(r1 + 1, t.tx.payment.amount.token.scalar()); put_u(r1 + 2, t.tx.payment.amount.amount);
-            r1[3] = pk[0]; r1[4] = pk[1];
-            size_t w = 0;
-            auto fr = [&](const Fr &v) { canon_out(r2 + (w++), v); };
-            auto u = [&](uint64_t v) { put_u(r2 + (w++), v); };
-            u(t.account_index); u(t.token_index); u(t.before.tx_nonce); u(t.before.withdraw_nonce); fr(t.before.address.x); fr(t.before.address.y);
-            fr(t.before_balances_hash); fr(t.before_balance.token.scalar()); u(t.before_balance.amount);
-            for (const Fr &v : t.balance_proof) fr(v);
-            for (const Fr &v : t.proof) fr(v);
-            if (w != w2) return BZK_ERR_BAD_ARG;
-            // revealed row {enabled, token, amount, H(pk)} (deposit_circuit.rs: the calldata of a deposit is the hash of its MPN key)
-            rv[0] = r1[0]; rv[1] = r1[1]; rv[2] = r1[2]; canon_out(rv + 3, t.enabled ? cd[e++] : Fr::zero());
-            canon_out(roots_out + s, roots[s]);
-        }
-        return BZK_OK;
+        BZK_TRY(finish(2, d.pk_hash));
+        slot_roots(deposits, k.state, k.next_state, enabled_roots, d.roots);
+        return write_deposit_rows(deposits, d, A, T, raws1, raws2, roots_out, reveal);
     }
-    const uint32_t w2 = 12 + 6 * T + 3 * A;
     std::vector<WithdrawTransition> withdraws;
     if (!padded(k.withdraws, k.config.log4_withdraw_batch, null_withdraw(A, T), withdraws)) return BZK_ERR_BAD_ARG;
-    std::vector<bzk_fr> pks(withdraws.size() * 2);
+    d.keys.resize(withdraws.size());
+    d.fingerprint.assign(withdraws.size(), Fr::zero());
     for (size_t s = 0; s < withdraws.size(); s++) {
         const WithdrawTransition &t = withdraws[s];
         if (!proofs_shaped(t.proof, A) || !proofs_shaped(t.token_balance_proof, T) || !proofs_shaped(t.fee_balance_proof, T)) return BZK_ERR_BAD_ARG;
-        BZK_TRY(rc.decompress(t.tx.mpn_address, pks.data() + 2 * s));
+        BZK_TRY(rc.decompress(t.tx.mpn_address, &d.keys[s]));
         if (!t.enabled) continue;
         jobs.push_back(RootJob{&t.before, t.before_token_hash, t.account_index, &t.proof});
+        enabled.push_back(s);
+        d.fingerprint[s] = withdraw_fingerprint(t.tx.payment);
         // calldata = H(pk, nonce, sig) (`verify_calldata`, /root/reference/src/core/transaction.rs:177-182)
-        cd_in.push_back(mont_of(pks[2 * s])); cd_in.push_back(mont_of(pks[2 * s + 1])); cd_in.push_back(Fr::from_u32(t.tx.nonce));
+        cd_in.push_back(d.keys[s].x); cd_in.push_back(d.keys[s].y); cd_in.push_back(Fr::from_u32(t.tx.nonce));
         cd_in.push_back(t.tx.sig.r.x); cd_in.push_back(t.tx.sig.r.y); cd_in.push_back(t.tx.sig.s);
     }
-    BZK_TRY(rc.entering_roots(jobs, A, enabled_roots));
-    slot_roots(withdraws, k.state, k.next_state, enabled_roots, roots);
-    cd.assign(jobs.size(), Fr::zero());
-    if (!jobs.empty()) BZK_TRY(rc.hash(6, cd_in.data(), jobs.size(), cd.data()));
-    size_t e = 0;
-    for (size_t s = 0; s < withdraws.size(); s++) {
-        const WithdrawTransition &t = withdraws[s];
-        const bzk_fr *pk = pks.data() + 2 * s;
-        const ContractWithdraw &p = t.tx.payment;
-        bzk_fr *r1 = raws1 + s * 12, *r2 = raws2 + s * w2, *rv = reveal + s * 7;
-        put_u(r1 + 0, t.enabled ? 1 : 0); canon_out(r1 + 1, p.amount.token.scalar()); put_u(r1 + 2, p.amount.amount);
-        canon_out(r1 + 3, p.fee.token.scalar()); put_u(r1 + 4, p.fee.amount);
-        canon_out(r1 + 5, t.enabled ? withdraw_fingerprint(p) : Fr::zero());
-        r1[6] = pk[0]; r1[7] = pk[1]; put_u(r1 + 8, t.tx.nonce);
-        canon_out(r1 + 9, t.tx.sig.r.x); canon_out(r1 + 10, t.tx.sig.r.y); canon_out(r1 + 11, t.tx.sig.s);
-        size_t w = 0;
-        auto fr = [&](const Fr &v) { canon_out(r2 + (w++), v); };
-        auto u = [&](uint64_t v) { put_u(r2 + (w++), v); };
-        u(t.account_index); u(t.token_index); u(t.fee_token_index); u(t.before.tx_nonce); u(t.before.withdraw_nonce);
-        fr(t.before.address.x); fr(t.before.address.y); fr(t.before_token_hash);
-        fr(t.before_token_balance.token.scalar()); u(t.before_token_balance.amount);
-        for (const Fr &v : t.token_balance_proof) fr(v);
-        fr(t.before_fee_balance.token.scalar()); u(t.before_fee_balance.amount);
-        for (const Fr &v : t.fee_balance_proof) fr(v);
-        for (const Fr &v : t.proof) fr(v);
-        if (w != w2) return BZK_ERR_BAD_ARG;
-        // revealed row {enabled, token, amount, fee token, fee, fingerprint, calldata}
-        for (int i = 0; i < 6; i++) rv[i] = r1[i];
-        canon_out(rv + 6, t.enabled ? cd[e++] : Fr::zero());
-        canon_out(roots_out + s, roots[s]);
-    }
-    return BZK_OK;
+    BZK_TRY(finish(6, d.calldata));
+    slot_roots(withdraws, k.state, k.next_state, enabled_roots, d.roots);
+    return write_withdraw_rows(withdraws, d, A, T, raws1, raws2, roots_out, reveal);
 }
 
 RowCtx host_rows(const bzk_poseidon_host *hasher, const bzk_fr *jj_d) {
@@ -728,10 +761,6 @@ int32_t bzk_mpn_post_solution_response_decode(const uint8_t *bytes, size_t len, 
 }  // extern "C"
 
 // ------------------------------------------------------------------------------------------------ prepare_works
-namespace {
-inline void canon_of(bzk_fr *out, const Fr &mont) { Fr c = mont.from_mont(); memcpy(out, c.l, 32); }
-}
-
 extern "C" {
 
 /* `mpn::prepare_works` (/root/reference/src/mpn/mod.rs:298-424) over the native ledger: on ONE fork of `state` (which is not
@@ -758,14 +787,13 @@ int32_t bzk_mpn_prepare_works(bzk_ctx *ctx, const bzk_mpn_state *state, const ui
     if (deposits_bytes && !dec_deposits(deposits_bytes, deposits_len, deposits)) return BZK_ERR_BAD_ARG;
     if (withdraws_bytes && !dec_withdraws(withdraws_bytes, withdraws_len, withdraws)) return BZK_ERR_BAD_ARG;
     if (updates_bytes && !dec_txs(updates_bytes, updates_len, updates)) return BZK_ERR_BAD_ARG;
-    const uint32_t A = config.log4_tree, T = config.log4_token;
     {
         bzk_fr root;
         uint64_t sz, cnt, pend;
         BZK_TRY(bzk_mpn_state_info(state, &root, &sz, &cnt, &pend));
         uint32_t shape[2] = {0, 0};
-        // the ledger must have the config's shape: the builders size their rows from the ledger's (A, T), the buffers below from the config's
-        if (bzk_mpn_state_shape(state, shape) != BZK_OK || shape[0] != A || shape[1] != T || config.log4_deposit_batch > 8 ||
+        // the ledger must have the config's shape: the builders size their proofs from the ledger's (A, T), a work's rows from the config's
+        if (bzk_mpn_state_shape(state, shape) != BZK_OK || shape[0] != config.log4_tree || shape[1] != config.log4_token || config.log4_deposit_batch > 8 ||
             config.log4_withdraw_batch > 8 || config.log4_update_batch > 8)
             return BZK_ERR_BAD_ARG;
     }
@@ -777,8 +805,8 @@ int32_t bzk_mpn_prepare_works(bzk_ctx *ctx, const bzk_mpn_state *state, const ui
             const MpnDeposit &d = deposits[k];
             bzk_mpn_deposit &o = dep_in[k];
             memset(&o, 0, sizeof o);
-            canon_of(&o.pk_x, d.mpn_address.x); o.pk_odd = d.mpn_address.odd ? 1 : 0;
-            canon_of(&o.token_id, d.payment.amount.token.scalar()); o.amount = d.payment.amount.amount;
+            fr_to_canon(&o.pk_x, d.mpn_address.x); o.pk_odd = d.mpn_address.odd ? 1 : 0;
+            fr_to_canon(&o.token_id, d.payment.amount.token.scalar()); o.amount = d.payment.amount.amount;
             const std::vector<uint8_t> src(d.payment.src, d.payment.src + 32);
             o.src_id = src_ids.emplace(src, src_ids.size() + 1).first->second;
         }
@@ -788,12 +816,12 @@ int32_t bzk_mpn_prepare_works(bzk_ctx *ctx, const bzk_mpn_state *state, const ui
         const MpnWithdraw &w = withdraws[k];
         bzk_mpn_withdraw &o = wd_in[k];
         memset(&o, 0, sizeof o);
-        canon_of(&o.pk_x, w.mpn_address.x); o.pk_odd = w.mpn_address.odd ? 1 : 0; o.nonce = w.nonce;
-        canon_of(&o.sig_rx, w.sig.r.x); canon_of(&o.sig_ry, w.sig.r.y); canon_of(&o.sig_s, w.sig.s);
-        canon_of(&o.amount_token_id, w.payment.amount.token.scalar()); canon_of(&o.fee_token_id, w.payment.fee.token.scalar());
-        canon_of(&o.fingerprint, withdraw_fingerprint(w.payment));
+        fr_to_canon(&o.pk_x, w.mpn_address.x); o.pk_odd = w.mpn_address.odd ? 1 : 0; o.nonce = w.nonce;
+        fr_to_canon(&o.sig_rx, w.sig.r.x); fr_to_canon(&o.sig_ry, w.sig.r.y); fr_to_canon(&o.sig_s, w.sig.s);
+        fr_to_canon(&o.amount_token_id, w.payment.amount.token.scalar()); fr_to_canon(&o.fee_token_id, w.payment.fee.token.scalar());
+        fr_to_canon(&o.fingerprint, withdraw_fingerprint(w.payment));
         o.amount = w.payment.amount.amount; o.fee = w.payment.fee.amount;
-        o.check_calldata = 1; canon_of(&o.calldata, w.payment.calldata);
+        o.check_calldata = 1; fr_to_canon(&o.calldata, w.payment.calldata);
     }
     std::vector<bzk_mpn_tx> up_in(updates.size());
     for (size_t k = 0; k < updates.size(); k++) {
@@ -802,16 +830,16 @@ int32_t bzk_mpn_prepare_works(bzk_ctx *ctx, const bzk_mpn_state *state, const ui
         memset(&o, 0, sizeof o);
         o.nonce = t.nonce; o.amount = t.amount.amount; o.fee = t.fee.amount;
         o.src_pk_odd = t.src.odd ? 1 : 0; o.dst_pk_odd = t.dst.odd ? 1 : 0;
-        canon_of(&o.src_pk_x, t.src.x); canon_of(&o.dst_pk_x, t.dst.x);
-        canon_of(&o.amount_token_id, t.amount.token.scalar()); canon_of(&o.fee_token_id, t.fee.token.scalar());
-        canon_of(&o.sig_rx, t.sig.r.x); canon_of(&o.sig_ry, t.sig.r.y); canon_of(&o.sig_s, t.sig.s);
+        fr_to_canon(&o.src_pk_x, t.src.x); fr_to_canon(&o.dst_pk_x, t.dst.x);
+        fr_to_canon(&o.amount_token_id, t.amount.token.scalar()); fr_to_canon(&o.fee_token_id, t.fee.token.scalar());
+        fr_to_canon(&o.sig_rx, t.sig.r.x); fr_to_canon(&o.sig_ry, t.sig.r.y); fr_to_canon(&o.sig_s, t.sig.s);
     }
     // ---- the batches, on one fork
     bzk_mpn_state *fork = nullptr;
     BZK_TRY(bzk_mpn_state_clone(state, &fork));
     std::vector<Work> works;
     int32_t st = BZK_OK;
-    auto finish = [&](Work &w, const bzk_fr public3[3], uint32_t kind) {
+    auto finish = [&](Work &w, const bzk_fr public3[3], uint32_t kind) -> Work && {
         w.config = config; w.height = height; w.kind = kind;
         Fr v[3];
         for (int i = 0; i < 3; i++) { memcpy(v[i].l, public3 + i, 32); v[i] = v[i].to_mont(); }
@@ -823,48 +851,29 @@ int32_t bzk_mpn_prepare_works(bzk_ctx *ctx, const bzk_mpn_state *state, const ui
         memcpy(rt.l, &root, 32);
         w.new_root_hash = rt.to_mont(); w.new_root_size = sz;
         w.reward = rewards[kind];
+        return std::move(w);
+    };
+    // a batch's transitions carry the transaction they were made from, as it came in
+    auto add = [&](auto &bt, const auto &inputs, auto &into) {
+        for (size_t i = 0; i < bt.t.size(); i++) { bt.t[i].tx = inputs[bt.from[i]]; into.push_back(std::move(bt.t[i])); }
     };
     for (uint64_t b = 0; st == BZK_OK && b < config.n_deposit_batches; b++) {
-        const uint64_t slots = 1ull << (2 * config.log4_deposit_batch);
-        std::vector<bzk_fr> r1(slots * 5), r2(slots * (9 + 3 * T + 3 * A)), roots(slots), rev(slots * 4);
-        bzk_fr pub[3];
-        uint64_t n_acc = 0;
-        DepositSink sink;
-        st = mpn_deposit_build_impl(ctx, fork, dep_in.data(), dep_in.size(), config.log4_deposit_batch, r1.data(), r2.data(), roots.data(), rev.data(), nullptr,
-                                    pub, &n_acc, &sink);
-        if (st != BZK_OK) break;
+        Built<DepositTransition> bt;
         Work w;
-        for (size_t i = 0; i < sink.t.size(); i++) { sink.t[i].tx = deposits[sink.from[i]]; w.deposits.push_back(std::move(sink.t[i])); }
-        finish(w, pub, KIND_DEPOSIT);
-        works.push_back(std::move(w));
+        st = mpn_deposit_build_impl(ctx, fork, dep_in.data(), dep_in.size(), config.log4_deposit_batch, &bt);
+        if (st == BZK_OK) { add(bt, deposits, w.deposits); works.push_back(finish(w, bt.public3, KIND_DEPOSIT)); }
     }
     for (uint64_t b = 0; st == BZK_OK && b < config.n_withdraw_batches; b++) {
-        const uint64_t slots = 1ull << (2 * config.log4_withdraw_batch);
-        std::vector<bzk_fr> r1(slots * 12), r2(slots * (12 + 6 * T + 3 * A)), roots(slots), rev(slots * 7);
-        bzk_fr pub[3];
-        uint64_t n_acc = 0;
-        WithdrawSink sink;
-        st = mpn_withdraw_build_impl(ctx, fork, wd_in.data(), wd_in.size(), config.log4_withdraw_batch, r1.data(), r2.data(), roots.data(), rev.data(), nullptr,
-                                     pub, &n_acc, &sink);
-        if (st != BZK_OK) break;
+        Built<WithdrawTransition> bt;
         Work w;
-        for (size_t i = 0; i < sink.t.size(); i++) { sink.t[i].tx = withdraws[sink.from[i]]; w.withdraws.push_back(std::move(sink.t[i])); }
-        finish(w, pub, KIND_WITHDRAW);
-        works.push_back(std::move(w));
+        st = mpn_withdraw_build_impl(ctx, fork, wd_in.data(), wd_in.size(), config.log4_withdraw_batch, &bt);
+        if (st == BZK_OK) { add(bt, withdraws, w.withdraws); works.push_back(finish(w, bt.public3, KIND_WITHDRAW)); }
     }
     for (uint64_t b = 0; st == BZK_OK && b < config.n_update_batches; b++) {
-        const uint64_t slots = 1ull << (2 * config.log4_update_batch);
-        std::vector<bzk_fr> raws(slots * (32 + 9 * T + 6 * A)), ext(slots * 2);
-        bzk_fr pub[3];
-        uint64_t n_acc = 0;
-        UpdateSink sink;
-        st = mpn_update_build_impl(ctx, fork, up_in.data(), up_in.size(), config.log4_update_batch, fee_token, raws.data(), ext.data(), nullptr, pub, &n_acc,
-                                   &sink);
-        if (st != BZK_OK) break;
+        Built<UpdateTransition> bt;
         Work w;
-        for (size_t i = 0; i < sink.t.size(); i++) { sink.t[i].tx = updates[sink.from[i]]; w.updates.push_back(std::move(sink.t[i])); }
-        finish(w, pub, KIND_UPDATE);
-        works.push_back(std::move(w));
+        st = mpn_update_build_impl(ctx, fork, up_in.data(), up_in.size(), config.log4_update_batch, fee_token, &bt);
+        if (st == BZK_OK) { add(bt, updates, w.updates); works.push_back(finish(w, bt.public3, KIND_UPDATE)); }
     }
     if (st != BZK_OK) { bzk_mpn_state_free(fork); return st; }
     Writer out;

@@ -18,14 +18,23 @@
 #include "common.cuh"
 
 namespace bzk {
-namespace wire {
 
-inline Fr fr_of_u64(uint64_t v) {   // Montgomery
+inline Fr fr_from_u64(uint64_t v) {   // Montgomery
     Fr a = Fr::zero();
     a.l[0] = (uint32_t)v;
     a.l[1] = (uint32_t)(v >> 32);
     return a.to_mont();
 }
+inline void fr_to_canon(bzk_fr *out, const Fr &mont) { const Fr c = mont.from_mont(); memcpy(out, c.l, 32); }
+
+// Widths of the circuits' rows (elements per slot): UpdateCircuit's raws; the deposit / withdraw circuits' phase-1 raws, phase-2
+// raws and revealed rows.
+inline uint32_t update_raw_width(uint32_t A, uint32_t T) { return 32 + 9 * T + 6 * A; }
+struct DwWidths { uint32_t raw1, raw2, reveal; };
+inline DwWidths deposit_widths(uint32_t A, uint32_t T) { return {5, 9 + 3 * T + 3 * A, 4}; }
+inline DwWidths withdraw_widths(uint32_t A, uint32_t T) { return {12, 12 + 6 * T + 3 * A, 7}; }
+
+namespace wire {
 
 struct ContractId {          // TokenId / ContractId::{Null, Ziesha, Custom(scalar)}
     uint32_t tag = 0;
@@ -45,11 +54,11 @@ struct PointW { Fr x = Fr::zero(), y = Fr::zero(); };             // jubjub::Poi
 struct PubKey { Fr x = Fr::zero(); bool odd = false; };           // jubjub::PublicKey(PointCompressed(x, is_odd))
 struct Sig { PointW r; Fr s = Fr::zero(); };                      // jubjub::Signature
 struct Account {
-    uint32_t tx_nonce = 0, withdraw_nonce = 0;
+    uint64_t tx_nonce = 0, withdraw_nonce = 0;                    // u32 on the wire
     PointW address;
     std::vector<std::pair<uint64_t, Money>> tokens;               // HashMap<u64, Money>, arrival order
 };
-struct MpnTx { uint32_t nonce = 0; PubKey src, dst; Money amount, fee; Sig sig; };
+struct MpnTx { uint64_t nonce = 0; PubKey src, dst; Money amount, fee; Sig sig; };   // nonce: u32 on the wire
 struct ContractDeposit {
     std::string memo;
     ContractId contract_id;
@@ -194,17 +203,54 @@ Fr withdraw_fingerprint(const ContractWithdraw &p);
 
 }  // namespace wire
 
-// The transition builders of csrc/mpn_host.cu with an optional sink for the reference's transition structs (`tx` left empty:
-// `from[i]` = index of the input the i-th transition was made from) — what `prepare_works` puts on the wire.
-struct UpdateSink { std::vector<wire::UpdateTransition> t; std::vector<uint64_t> from; };
-struct DepositSink { std::vector<wire::DepositTransition> t; std::vector<uint64_t> from; };
-struct WithdrawSink { std::vector<wire::WithdrawTransition> t; std::vector<uint64_t> from; };
+// `{Update,Deposit,Withdraw}Transition::null` (/root/reference/src/mpn/mod.rs:440-537): what a batch is padded with — the builders
+// and a work carry only the transitions made, the circuit always has 4^B slots
+wire::UpdateTransition null_update(uint32_t A, uint32_t T);
+wire::DepositTransition null_deposit(uint32_t A, uint32_t T);
+wire::WithdrawTransition null_withdraw(uint32_t A, uint32_t T);
+// a batch padded to its 4^B slots; false when it holds more transitions than that
+template <class Tr>
+bool padded(const std::vector<Tr> &ts, uint32_t log4_batch, const Tr &null, std::vector<Tr> &out) {
+    if (log4_batch > 8) return false;
+    const size_t slots = (size_t)1 << (2 * log4_batch);
+    if (ts.size() > slots) return false;
+    out = ts;
+    out.resize(slots, null);
+    return true;
+}
+
+// What a slot's circuit rows need besides its transition, one entry per slot of the padded batch (Montgomery): the state root
+// entering the slot, the decompressed key of its transaction ((0, -1) for a null slot: `PublicKey::default().decompress()`),
+// and per kind the deposit's H(pk), the withdrawal's fingerprint and calldata hash (zero where the slot is not enabled).
+struct SlotData { std::vector<Fr> roots; std::vector<wire::PointW> keys; std::vector<Fr> pk_hash, fingerprint, calldata; };
+
+// The one writer of each circuit's rows (canonical scalars), from a padded batch and its SlotData; the builders' C ABI and the
+// work decoder both call it.  Update: raws[4^B][update_raw_width], ext[4^B][2] = {fee token, entering root}.  Deposit / withdraw:
+// raws1, raws2, the entering roots and the revealed rows ({deposit,withdraw}_widths).
+int32_t write_update_rows(const std::vector<wire::UpdateTransition> &ts, const SlotData &d, uint32_t A, uint32_t T, const Fr &fee_token, bzk_fr *raws,
+                          bzk_fr *ext);
+int32_t write_deposit_rows(const std::vector<wire::DepositTransition> &ts, const SlotData &d, uint32_t A, uint32_t T, bzk_fr *raws1, bzk_fr *raws2,
+                           bzk_fr *roots, bzk_fr *reveal);
+int32_t write_withdraw_rows(const std::vector<wire::WithdrawTransition> &ts, const SlotData &d, uint32_t A, uint32_t T, bzk_fr *raws1, bzk_fr *raws2,
+                            bzk_fr *roots, bzk_fr *reveal);
+// a slot's revealed row (Montgomery): deposit {enabled, token, amount, H(pk)}, withdraw {enabled, token, amount, fee token, fee,
+// fingerprint, calldata}; the root of their list is the batch's aux_data
+void deposit_reveal(const wire::DepositTransition &t, const SlotData &d, size_t slot, Fr out[4]);
+void withdraw_reveal(const wire::WithdrawTransition &t, const SlotData &d, size_t slot, Fr out[7]);
+
+// The transition builders of csrc/mpn_host.cu: the transitions of the accepted inputs (`tx` as the builder saw it; from[i] = index
+// of the input the i-th transition was made from), their SlotData over the 4^B slots, and {state, aux_data, next_state} (canonical).
+template <class Tr>
+struct Built {
+    std::vector<Tr> t;
+    std::vector<uint64_t> from;
+    SlotData d;
+    bzk_fr public3[3];
+};
 int32_t mpn_update_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_tx *txs, uint64_t n_txs, uint32_t log4_batch, const bzk_fr *fee_token_canon,
-                              bzk_fr *raws, bzk_fr *ext, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted, UpdateSink *sink);
-int32_t mpn_deposit_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_deposit *deps, uint64_t n_deps, uint32_t log4_batch, bzk_fr *raws1,
-                               bzk_fr *raws2, bzk_fr *roots, bzk_fr *reveal, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted,
-                               DepositSink *sink);
-int32_t mpn_withdraw_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_withdraw *wds, uint64_t n_wds, uint32_t log4_batch, bzk_fr *raws1,
-                                bzk_fr *raws2, bzk_fr *roots, bzk_fr *reveal, uint8_t *accepted, bzk_fr public3[3], uint64_t *n_accepted,
-                                WithdrawSink *sink);
+                              Built<wire::UpdateTransition> *out);
+int32_t mpn_deposit_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_deposit *deps, uint64_t n_deps, uint32_t log4_batch,
+                               Built<wire::DepositTransition> *out);
+int32_t mpn_withdraw_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_withdraw *wds, uint64_t n_wds, uint32_t log4_batch,
+                                Built<wire::WithdrawTransition> *out);
 }  // namespace bzk
