@@ -119,6 +119,9 @@ SIGNATURES = {
     "bzk_jubjub_eddsa_verify_batch": (_i32, [_vp, _vp, _vp, _sz, _vp, _vp]),
     "bzk_mpn_tx_verify_batch": (_i32, [_vp, _vp, _vp, _sz, _vp, _vp]),
     "bzk_mpn_signatures_verify_bytes": (_i32, [_vp, _vp, _u32, _vp, _sz, _vp, _sz, _vp, _vp]),
+    "bzk_ed25519_verify": (_i32, [_vp, _vp, _sz, _vp]),
+    "bzk_ed25519_verify_batch": (_i32, [_vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "bzk_mpn_deposits_verify_bytes": (_i32, [_vp, _vp, _sz, _vp, _sz, _vp, _vp]),
     "bzk_mpn_deposit_build": (_i32, [_vp, _vp, _vp, _u64, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bzk_mpn_withdraw_build": (_i32, [_vp, _vp, _vp, _u64, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bzk_mpn_dw_witness": (_i32, [_vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp]),

@@ -412,3 +412,15 @@ class HostPoseidon:
             self.free()
         except Exception:
             pass
+
+
+def ed25519_verify(pk, msg, sig):
+    """`Ed25519::verify` (src/crypto/ed25519.rs:81-83 of the reference, ed25519-dalek 1.x `PublicKey::verify`) on the host, no
+    context and no GPU (include/bzk.h, bzk_ed25519_verify): 32-byte key, message, 64-byte signature in, bool out"""
+    pk, msg, sig = bytes(pk), bytes(msg), bytes(sig)
+    if len(pk) != 32 or len(sig) != 64:
+        raise ValueError("an ed25519 key is 32 bytes and a signature 64")
+    st = _lib.load().bzk_ed25519_verify(pk, msg, len(msg), sig)
+    if st < 0:
+        raise BzkError(st, "ed25519_verify")
+    return bool(st)

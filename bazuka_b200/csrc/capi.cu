@@ -177,6 +177,7 @@ int32_t bzk_ctx_destroy(bzk_ctx *ctx) {
     for (auto &t : ctx->ntt) { if (t.d_fwd) cudaFree(t.d_fwd); if (t.d_inv) cudaFree(t.d_inv); }
     if (ctx->d_gpow) cudaFree(ctx->d_gpow);
     if (ctx->d_jj_table) cudaFree(ctx->d_jj_table);
+    if (ctx->d_ed_table) cudaFree(ctx->d_ed_table);
     if (ctx->ws) cudaFree(ctx->ws);
     if (ctx->stage) cudaFree(ctx->stage);
     if (ctx->pinned) cudaFreeHost(ctx->pinned);

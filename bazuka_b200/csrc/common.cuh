@@ -97,6 +97,8 @@ struct bzk_ctx {
     // batch signature check (jubjub.cu)
     void *d_jj_table = nullptr;
     bzk::Fr jj_table_d{};
+    // Ed25519 fixed-base table of B (ed25519.cuh, kJJFixedEntries EdNiels25519), made by the first batch Ed25519 check (ed25519.cu)
+    void *d_ed_table = nullptr;
 };
 
 // A base vector, in one of two places.  On the device, `d` holds it; after bzk_g*_bases_precompute `d` holds tab_T levels

@@ -20,51 +20,56 @@ BZK_HD bool jj_on_curve(const Fr &x, const Fr &y, const Fr &d) {
     return (y2 - x2) == (Fr::one() + d * x2 * y2);
 }
 
+// The group law below is written once over the field F of any twisted Edwards curve with a = -1 and a non-square d, where it
+// is complete: JubJub (F = Fr) here, Ed25519 (F = Fe<P25519Params>) in ed25519.cuh.
 // extended coordinates: x = X/Z, y = Y/Z, xy = T/Z (Z never vanishes on the curve: the formulas below are complete)
-struct JJ { Fr x, y, t, z; };
+template <class F> struct EdExt { F x, y, t, z; };
 // an addend in the form the addition consumes: (Y - X, Y + X, 2d T, 2Z)
-struct JJCached { Fr ymx, ypx, t2d, z2; };
-// an affine addend (Z = 1): (y - x, y + x, 2d x y) — the fixed-base table's entries
-struct JJNiels { Fr ymx, ypx, t2d; };
+template <class F> struct EdCached { F ymx, ypx, t2d, z2; };
+// an affine addend (Z = 1): (y - x, y + x, 2d x y) — the fixed-base tables' entries
+template <class F> struct EdNiels { F ymx, ypx, t2d; };
+using JJ = EdExt<Fr>;
+using JJCached = EdCached<Fr>;
+using JJNiels = EdNiels<Fr>;
 
-BZK_HD JJ jj_identity() { return JJ{Fr::zero(), Fr::one(), Fr::zero(), Fr::one()}; }
-BZK_HD JJ jj_from_affine(const Fr &x, const Fr &y) { return JJ{x, y, x * y, Fr::one()}; }
-BZK_HD JJCached jj_cached(const JJ &p, const Fr &d2) { return JJCached{p.y - p.x, p.y + p.x, p.t * d2, p.z.dbl()}; }
+template <class F> BZK_HD EdExt<F> jj_identity() { return EdExt<F>{F::zero(), F::one(), F::zero(), F::one()}; }
+template <class F> BZK_HD EdExt<F> jj_from_affine(const F &x, const F &y) { return EdExt<F>{x, y, x * y, F::one()}; }
+template <class F> BZK_HD EdCached<F> jj_cached(const EdExt<F> &p, const F &d2) { return EdCached<F>{p.y - p.x, p.y + p.x, p.t * d2, p.z.dbl()}; }
 
 // unified addition, a = -1 ("add-2008-hwcd-3"): 9 products
-BZK_HD JJ jj_add(const JJ &p, const JJCached &q) {
-    const Fr a = (p.y - p.x) * q.ymx, b = (p.y + p.x) * q.ypx, c = p.t * q.t2d, d = p.z * q.z2;
-    const Fr e = b - a, f = d - c, g = d + c, h = b + a;
-    return JJ{e * f, g * h, e * h, f * g};
+template <class F> BZK_HD EdExt<F> jj_add(const EdExt<F> &p, const EdCached<F> &q) {
+    const F a = (p.y - p.x) * q.ymx, b = (p.y + p.x) * q.ypx, c = p.t * q.t2d, d = p.z * q.z2;
+    const F e = b - a, f = d - c, g = d + c, h = b + a;
+    return EdExt<F>{e * f, g * h, e * h, f * g};
 }
 // the same with Z2 = 1: 7 products
-BZK_HD JJ jj_add(const JJ &p, const JJNiels &q) {
-    const Fr a = (p.y - p.x) * q.ymx, b = (p.y + p.x) * q.ypx, c = p.t * q.t2d, d = p.z.dbl();
-    const Fr e = b - a, f = d - c, g = d + c, h = b + a;
-    return JJ{e * f, g * h, e * h, f * g};
+template <class F> BZK_HD EdExt<F> jj_add(const EdExt<F> &p, const EdNiels<F> &q) {
+    const F a = (p.y - p.x) * q.ymx, b = (p.y + p.x) * q.ypx, c = p.t * q.t2d, d = p.z.dbl();
+    const F e = b - a, f = d - c, g = d + c, h = b + a;
+    return EdExt<F>{e * f, g * h, e * h, f * g};
 }
 // doubling, a = -1 ("dbl-2008-hwcd"): 8 products
-BZK_HD JJ jj_dbl(const JJ &p) {
-    const Fr a = p.x.sqr(), b = p.y.sqr(), c = p.z.sqr().dbl();
-    const Fr e = (p.x + p.y).sqr() - a - b, g = b - a, f = g - c, h = (a + b).neg();
-    return JJ{e * f, g * h, e * h, f * g};
+template <class F> BZK_HD EdExt<F> jj_dbl(const EdExt<F> &p) {
+    const F a = p.x.sqr(), b = p.y.sqr(), c = p.z.sqr().dbl();
+    const F e = (p.x + p.y).sqr() - a - b, g = b - a, f = g - c, h = (a + b).neg();
+    return EdExt<F>{e * f, g * h, e * h, f * g};
 }
 // the same group element (projective equality of X/Z and Y/Z)
-BZK_HD bool jj_equal(const JJ &p, const JJ &q) { return p.x * q.z == q.x * p.z && p.y * q.z == q.y * p.z; }
+template <class F> BZK_HD bool jj_equal(const EdExt<F> &p, const EdExt<F> &q) { return p.x * q.z == q.x * p.z && p.y * q.z == q.y * p.z; }
 
-// [k] P for a plain 256-bit little-endian k (any k: no reduction), 4-bit unsigned windows MSB first: 256 doublings and 64
-// additions of a per-call table of [0..15] P
-BZK_HD JJ jj_mul(const JJ &p, const Fr &k, const Fr &d2) {
-    JJCached tab[16];
-    tab[0] = jj_cached(jj_identity(), d2);
+// [k] P for a plain 256-bit little-endian k (any k: no reduction; K is any 8-limb Fe, only its limbs are read), 4-bit unsigned
+// windows MSB first: 256 doublings and 64 additions of a per-call table of [0..15] P
+template <class F, class K> BZK_HD EdExt<F> jj_mul(const EdExt<F> &p, const K &k, const F &d2) {
+    EdCached<F> tab[16];
+    tab[0] = jj_cached(jj_identity<F>(), d2);
     tab[1] = jj_cached(p, d2);
-    JJ cur = p;
+    EdExt<F> cur = p;
 #pragma unroll 1
     for (int i = 2; i < 16; i++) {
         cur = jj_add(cur, tab[1]);
         tab[i] = jj_cached(cur, d2);
     }
-    JJ acc = jj_identity();
+    EdExt<F> acc = jj_identity<F>();
 #pragma unroll 1
     for (int w = 63; w >= 0; w--) {
         acc = jj_dbl(jj_dbl(jj_dbl(jj_dbl(acc))));
@@ -73,15 +78,44 @@ BZK_HD JJ jj_mul(const JJ &p, const Fr &k, const Fr &d2) {
     return acc;
 }
 
-// The fixed-base table of BASE: kJJFixedWindows windows of 8 bits, entry [j][v] = [v * 2^(8j)] BASE (v = 0: the identity), so
-// that [k] BASE is one mixed addition per byte of k.  786 KB on the device, built once per context (jubjub.cu).
+// A fixed-base table: kJJFixedWindows windows of 8 bits, entry [j][v] = [v * 2^(8j)] G (v = 0: the identity), so that [k] G is
+// one mixed addition per byte of k.  786 KB on the device, built once per context (jubjub.cu: G = BASE, ed25519.cu: G = B).
 constexpr int kJJFixedWindows = 32;
 constexpr int kJJFixedEntries = kJJFixedWindows * 256;
-BZK_HD JJ jj_mul_fixed(const JJNiels *tab, const Fr &k) {
-    JJ acc = jj_identity();
+template <class F, class K> BZK_HD EdExt<F> jj_mul_fixed(const EdNiels<F> *tab, const K &k) {
+    EdExt<F> acc = jj_identity<F>();
 #pragma unroll 1
     for (int j = 0; j < kJJFixedWindows; j++) acc = jj_add(acc, tab[j * 256 + ((k.l[j >> 2] >> (8 * (j & 3))) & 255u)]);
     return acc;
+}
+
+// host: the fixed-base table of the affine point (gx, gy) on the curve with this d (Montgomery); entries normalised to affine
+// with one batched inversion
+template <class F> inline std::vector<EdNiels<F>> ed_fixed_base_table(const F &gx, const F &gy, const F &d) {
+    const F d2 = d.dbl();
+    std::vector<EdExt<F>> pts(kJJFixedEntries);
+    EdExt<F> row = jj_from_affine(gx, gy);   // [2^(8j)] G
+    for (int j = 0; j < kJJFixedWindows; j++) {
+        const EdCached<F> step = jj_cached(row, d2);
+        EdExt<F> cur = jj_identity<F>();
+        for (int v = 0; v < 256; v++) {
+            pts[j * 256 + v] = cur;
+            cur = jj_add(cur, step);
+        }
+        row = cur;
+    }
+    std::vector<F> prefix(kJJFixedEntries);
+    F acc = F::one();
+    for (int i = 0; i < kJJFixedEntries; i++) { prefix[i] = acc; acc = acc * pts[i].z; }
+    F inv = acc.inv_gcd();
+    std::vector<EdNiels<F>> out(kJJFixedEntries);
+    for (int i = kJJFixedEntries - 1; i >= 0; i--) {
+        const F zi = inv * prefix[i];
+        inv = inv * pts[i].z;
+        const F x = pts[i].x * zi, y = pts[i].y * zi;
+        out[i] = EdNiels<F>{y - x, y + x, x * y * d2};
+    }
+    return out;
 }
 
 // BASE (curve.rs:146-164), Montgomery
@@ -93,34 +127,11 @@ BZK_HD void jj_base(Fr *x, Fr *y) {
     *y = Fr::from_u32(18);
 }
 
-// host: the fixed-base table for the curve with this d (Montgomery); entries normalised to affine with one batched inversion
+// host: the fixed-base table of BASE for the curve with this d (Montgomery)
 inline std::vector<JJNiels> jj_fixed_base_table(const Fr &d) {
-    const Fr d2 = d.dbl();
     Fr bx, by;
     jj_base(&bx, &by);
-    std::vector<JJ> pts(kJJFixedEntries);
-    JJ row = jj_from_affine(bx, by);   // [2^(8j)] BASE
-    for (int j = 0; j < kJJFixedWindows; j++) {
-        const JJCached step = jj_cached(row, d2);
-        JJ cur = jj_identity();
-        for (int v = 0; v < 256; v++) {
-            pts[j * 256 + v] = cur;
-            cur = jj_add(cur, step);
-        }
-        row = cur;
-    }
-    std::vector<Fr> prefix(kJJFixedEntries);
-    Fr acc = Fr::one();
-    for (int i = 0; i < kJJFixedEntries; i++) { prefix[i] = acc; acc = acc * pts[i].z; }
-    Fr inv = acc.inv_gcd();
-    std::vector<JJNiels> out(kJJFixedEntries);
-    for (int i = kJJFixedEntries - 1; i >= 0; i--) {
-        const Fr zi = inv * prefix[i];
-        inv = inv * pts[i].z;
-        const Fr x = pts[i].x * zi, y = pts[i].y * zi;
-        out[i] = JJNiels{y - x, y + x, x * y * d2};
-    }
-    return out;
+    return ed_fixed_base_table(bx, by, d);
 }
 
 // Fr square root (Tonelli-Shanks, r - 1 = 2^32 q with q odd, 7 a non-residue); false when none exists.  One 223-bit power:

@@ -144,9 +144,13 @@ void dec_address(Reader &r, uint8_t out[32]) {   // ed25519 key (ext): serialize
     const uint8_t *p = r.take(32);
     if (p) memcpy(out, p, 32);
 }
-void enc_contract_deposit(Writer &w, const ContractDeposit &p) {
+// the fields before the Option<Signature> tag
+void enc_contract_deposit_head(Writer &w, const ContractDeposit &p) {
     w.bytes(p.memo.data(), p.memo.size()); enc_contract_id(w, p.contract_id); w.u32(p.circuit_id); w.fr(p.calldata);
     w.bytes(p.src, 32); enc_money(w, p.amount); enc_money(w, p.fee); w.u32(p.nonce);
+}
+void enc_contract_deposit(Writer &w, const ContractDeposit &p) {
+    enc_contract_deposit_head(w, p);
     w.u8(p.has_sig ? 1 : 0);
     if (p.has_sig) w.bytes(p.sig.data(), p.sig.size());
 }
@@ -235,6 +239,11 @@ void dec_config(Reader &r, Config &c) {
     for (int k = 0; k < 3; k++) dec_vk(r, c.vk[k]);
 }
 }  // namespace
+
+void enc_contract_deposit_unsigned(Writer &w, const ContractDeposit &p) {
+    enc_contract_deposit_head(w, p);
+    w.u8(0);
+}
 
 void enc_contract_withdraw(Writer &w, const ContractWithdraw &p) {
     w.bytes(p.memo.data(), p.memo.size()); enc_contract_id(w, p.contract_id); w.u32(p.circuit_id); w.fr(p.calldata);

@@ -191,6 +191,10 @@ void enc_contract_withdraw(Writer &w, const ContractWithdraw &p);
 // or an unreduced scalar
 bool dec_withdraws(const uint8_t *b, size_t n, std::vector<MpnWithdraw> &out);
 bool dec_txs(const uint8_t *b, size_t n, std::vector<MpnTx> &out);
+bool dec_deposits(const uint8_t *b, size_t n, std::vector<MpnDeposit> &out);
+// bincode of the payment with sig = None: the message its ed25519 signature covers (`ContractDeposit::verify_signature`,
+// src/core/transaction.rs:192-201)
+void enc_contract_deposit_unsigned(Writer &w, const ContractDeposit &p);
 
 // sha3-256 (FIPS 202) — `Hasher::hash` of the reference (/root/reference/src/crypto/mod.rs, sha3::Sha3_256)
 void sha3_256(const uint8_t *data, size_t len, uint8_t out[32]);

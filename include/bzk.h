@@ -479,6 +479,34 @@ int32_t bzk_jubjub_eddsa_verify_batch(bzk_ctx *ctx, const bzk_fr *jubjub_d, cons
 int32_t bzk_mpn_tx_verify_batch(bzk_ctx *ctx, const bzk_fr *jubjub_d, const bzk_mpn_tx *txs, size_t n, uint8_t *ok, uint64_t *n_ok);
 int32_t bzk_mpn_signatures_verify_bytes(bzk_ctx *ctx, const bzk_fr *jubjub_d, uint32_t kind, const uint8_t *bytes, size_t len, uint8_t *ok,
                                         size_t cap, uint64_t *n, uint64_t *n_ok);
+/* ------------------------------------------------------------------ Ed25519 signature checks (L1: deposits, transactions)
+ * `Ed25519::verify` (src/crypto/ed25519.rs:81-83): ed25519-dalek 1.x `PublicKey::verify`, the non-strict, cofactorless check.
+ * For pk (32 B), sig = R || s (64 B) and message M the verdict is 1 iff
+ *   s (little-endian) < l = 2^252 + 27742317777372353535851937790883648493 (s is never reduced; bit 255 set gives 0);
+ *   pk decompresses as curve25519-dalek 3.x does: y = the low 255 bits taken mod p (non-canonical y accepted), x =
+ *     sqrt_ratio_i(y^2 - 1, d y^2 + 1) exists, the non-negative root negated when bit 255 is set ("-0" accepted); small-order
+ *     and mixed-order keys are accepted;
+ *   k = SHA-512(R || pk || M) as a 512-bit little-endian integer mod l;
+ *   compress([k](-A) + [s]B) == R byte for byte, in the full group (no cofactor): a non-canonical, off-curve or "-0" R gives 0.
+ *   bzk_ed25519_verify              one signature on the host, no context: 1 accept, 0 reject, < 0 bad argument (pk or sig
+ *                                   NULL, msg NULL with len > 0)
+ *   bzk_ed25519_verify_batch        on the GPU, one thread per signature: pks n x 32 B, sigs n x 64 B, message i =
+ *                                   msgs[offsets[i] .. offsets[i+1]) with n + 1 offsets, offsets[0] = 0, non-decreasing (msgs
+ *                                   may be NULL when offsets[n] = 0).  The TransactionAndDelta arm: M = bincode(sig_state_excluded()),
+ *                                   src/core/transaction.rs:386-397
+ *   bzk_mpn_deposits_verify_bytes   `ContractDeposit::verify_signature` (src/core/transaction.rs:192-201) of each payment of a
+ *                                   bincode Vec<MpnDeposit>, the image bzk_mpn_prepare_works takes: M = bincode(payment with sig
+ *                                   = None); 0 where sig is None or not 64 bytes.  ok == NULL: only *n (the item count); cap < *n:
+ *                                   BZK_ERR_BAD_ARG
+ * ok[i] = 1 (accept) or 0 (reject); n_ok (optional) = the number accepted.  A rejected signature is a verdict: the call returns
+ * BZK_OK.  BZK_ERR_BAD_ARG (nothing written to ok): a null pointer with n > 0, bad offsets, a malformed image.  Synchronous on
+ * the context's stream.  Items go through the context's arena at most 2^18 items and 64 MiB of messages at a time (a longer
+ * single message goes alone), so device memory stays bounded for any batch; the context keeps a fixed-base table of B
+ * (786 KB), built on first use. */
+int32_t bzk_ed25519_verify(const uint8_t pk[32], const uint8_t *msg, size_t len, const uint8_t sig[64]);
+int32_t bzk_ed25519_verify_batch(bzk_ctx *ctx, const uint8_t *pks, const uint8_t *sigs, const uint8_t *msgs, const uint64_t *offsets, size_t n,
+                                 uint8_t *ok, uint64_t *n_ok);
+int32_t bzk_mpn_deposits_verify_bytes(bzk_ctx *ctx, const uint8_t *bytes, size_t len, uint8_t *ok, size_t cap, uint64_t *n, uint64_t *n_ok);
 int32_t bzk_mpn_update_build(bzk_ctx *ctx, bzk_mpn_state *state, const bzk_mpn_tx *txs, uint64_t n_txs, uint32_t log4_batch,
                              const bzk_fr *fee_token, bzk_fr *raws, bzk_fr *ext, uint8_t *accepted, bzk_fr public3[3],
                              uint64_t *n_accepted);
