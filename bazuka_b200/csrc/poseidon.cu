@@ -304,7 +304,8 @@ int32_t merkle4_build(bzk_ctx *ctx, Fr *d_nodes, uint32_t log4) {
     return BZK_OK;
 }
 int32_t merkle4_prove(bzk_ctx *ctx, const Fr *d_nodes, uint32_t log4, const uint64_t *d_idx, size_t m, Fr *d_proofs) {
-    if (log4 > 15 || (m && (!d_nodes || !d_idx || !d_proofs))) return BZK_ERR_BAD_ARG;
+    // a one-leaf tree (log4 = 0) has empty proofs: like merkle4_root, no proof buffer is needed then
+    if (log4 > 15 || (m && (!d_nodes || !d_idx || (log4 && !d_proofs)))) return BZK_ERR_BAD_ARG;
     if (m == 0 || log4 == 0) return BZK_OK;
     k_merkle4_prove<<<div_up(m * log4, 256), 256, 0, ctx->stream>>>(d_nodes, log4, d_idx, m, d_proofs);
     BZK_LAUNCHED(ctx);

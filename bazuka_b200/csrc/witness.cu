@@ -117,6 +117,13 @@ struct bzk_witness_program {
 };
 
 namespace bzk {
+// a field image is usable as it stands only below r: the device arithmetic assumes reduced operands
+static bool fr_image_below_r(const bzk_fr *v) {
+    Fr a;
+    memcpy(&a, v, sizeof(Fr));
+    return Fr::reduce_once(a) == a;
+}
+
 // the shape a driver must match before it hands rows to the interpreter (csrc/mpn_host.cu)
 void witness_program_shape(const bzk_witness_program *p, uint64_t *n_ops, uint32_t *n_raw, uint32_t *n_ext) {
     *n_ops = p->d.n_ops; *n_raw = p->d.n_raw; *n_ext = p->d.n_ext;
@@ -129,7 +136,13 @@ int32_t bzk_witness_program_upload(bzk_ctx *ctx, const int32_t *ops, uint64_t n_
                                    const int32_t *lc_slot, const int32_t *lc_coef, uint64_t n_terms, const bzk_fr *coefs,
                                    uint64_t n_coefs, uint32_t n_raw, uint32_t n_ext, const bzk_fr *jj_d, bzk_witness_program **out) {
     if (!ctx || !ops || !lc_ptr || !coefs || !jj_d || !out || !n_ops || !n_coefs || (n_terms && (!lc_slot || !lc_coef))) return BZK_ERR_BAD_ARG;
-    // validate on the host: the device interpreter trusts the program
+    // validate on the host: the device interpreter trusts the program.  It takes coefficient index 0 as one without
+    // reading coefs[0], so any other value there would make the device and the program's own meaning disagree.
+    Fr c0;
+    memcpy(&c0, coefs, sizeof(Fr));
+    if (c0 != Fr::one() || !fr_image_below_r(jj_d)) return BZK_ERR_BAD_ARG;
+    for (uint64_t k = 1; k < n_coefs; k++)
+        if (!fr_image_below_r(coefs + k)) return BZK_ERR_BAD_ARG;
     const uint64_t kSlotBlock0 = 1 + (uint64_t)n_ext;
     for (uint64_t j = 0; j < n_ops; j++) {
         const int32_t *op = ops + j * 6;

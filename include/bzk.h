@@ -571,7 +571,8 @@ int32_t bzk_mpn_circuit_program(const bzk_mpn_circuit *circuit, uint32_t which, 
  *   linear combination l = sum_{k in [lc_ptr[l], lc_ptr[l+1])} coefs[lc_coef[k]] * V[lc_slot[k]]
  *   (coefs[0] must be the constant one); slots: 0 = ONE, 1..n_ext = variables the block reads but does not
  *   define (update circuit: the fee token and the state root entering the slot), 1 + n_ext + j = block
- *   variable j.  coefs and jj_d (the curve's d) are Montgomery images.
+ *   variable j.  coefs and jj_d (the curve's d) are Montgomery images, each below r, and coefs[0] is the
+ *   Montgomery image of one; the upload refuses a program that breaks either rule (BZK_ERR_BAD_ARG).
  * bzk_witness_run_dev: raws[ntx][n_raw] and ext[ntx][n_ext] are CANONICAL host images (converted on the
  * device); writes the Montgomery values of slot t's variables to d_aux_out[t*n_ops + j]. */
 int32_t bzk_witness_program_upload(bzk_ctx *ctx, const int32_t *ops, uint64_t n_ops, const int32_t *lc_ptr, uint64_t n_lc,
