@@ -15,7 +15,7 @@ BZK_OK = 0
 ERRORS = {
     -1: "BZK_ERR_BAD_ARG", -2: "BZK_ERR_CUDA", -3: "BZK_ERR_OOM", -4: "BZK_ERR_NOT_ON_CURVE",
     -5: "BZK_ERR_NO_PARAMS", -6: "BZK_ERR_NO_DEVICE", -7: "BZK_ERR_UNSAT", -8: "BZK_ERR_BAD_ENCODING",
-    -9: "BZK_ERR_NOT_IN_SUBGROUP",
+    -9: "BZK_ERR_NOT_IN_SUBGROUP", -10: "BZK_ERR_REJECTED",
 }
 
 
@@ -89,6 +89,7 @@ SIGNATURES = {
     "bzk_r1cs_columns_dev": (_i32, [_vp, _vp, _u32, _vp, _vp]),
     "bzk_groth16_params_create": (_i32, [_vp] * 11 + [ct.POINTER(_vp)]),
     "bzk_groth16_params_free": (_i32, [_vp, _vp]),
+    "bzk_groth16_params_info": (_i32, [_vp] * 7),
     "bzk_groth16_prove": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "bzk_groth16_prove_dev": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "bzk_groth16_stage_ms": (_i32, [_vp, _vp]),
@@ -165,6 +166,10 @@ SIGNATURES = {
     "bzk_mpn_work_dw_rows_ctx": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bzk_mpn_prover_free": (_i32, [_vp, _vp]),
     "bzk_mpn_prover_prove_work": (_i32, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i32, _vp]),
+    "bzk_mpn_worker_create": (_i32, [_vp, _sz, _vp, _u32, _vp, _sz, _vp, _vp, ct.POINTER(_vp)]),
+    "bzk_mpn_worker_prove_response": (_i32, [_vp, _vp, _sz, _vp, _vp, ct.POINTER(_vp), ct.POINTER(_sz), _vp, _u64, ct.POINTER(_u64)]),
+    "bzk_mpn_worker_free": (_i32, [_vp]),
+    "bzk_mpn_worker_last_timing": (_i32, [_vp, _vp]),
     "bzk_witness_program_upload": (_i32, [_vp, _vp, _u64, _vp, _u64, _vp, _vp, _u64, _vp, _u64, _u32, _u32, _vp, ct.POINTER(_vp)]),
     "bzk_witness_program_free": (_i32, [_vp, _vp]),
     "bzk_witness_run_dev": (_i32, [_vp, _vp, _vp, _vp, _u64, _vp]),

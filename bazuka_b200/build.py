@@ -11,10 +11,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_obj")
 SO = os.path.join(HERE, "libbzk.so")
-SOURCES = ["msm_g2.cu", "msm_g1.cu", "groth16.cu", "poseidon.cu", "poseidon_host.cu", "ntt.cu", "verify.cu", "witness.cu", "mpn_host.cu", "mpn_wire.cu", "mpn_prover.cu", "mpn_circuit.cu", "params_io.cu", "jubjub.cu", "ed25519.cu", "capi.cu"]
+SOURCES = ["msm_g2.cu", "msm_g1.cu", "groth16.cu", "poseidon.cu", "poseidon_host.cu", "ntt.cu", "verify.cu", "witness.cu", "mpn_host.cu", "mpn_wire.cu", "mpn_prover.cu", "mpn_worker.cu", "mpn_circuit.cu", "params_io.cu", "jubjub.cu", "ed25519.cu", "capi.cu"]
 HEADERS = ["ff.cuh", "ec.cuh", "common.cuh", "msm_impl.cuh", "witness_core.cuh", "jubjub.cuh", "pairing.cuh", os.path.join("..", "..", "include", "bzk.h")]
 # headers only some sources include
-EXTRA_DEPS = {"mpn_wire.cu": ["mpn_wire.cuh"], "mpn_host.cu": ["mpn_wire.cuh", "hash_plan.cuh"], "poseidon.cu": ["hash_plan.cuh"], "mpn_prover.cu": ["mpn_wire.cuh"], "params_io.cu": ["params_io.cuh"], "groth16.cu": ["r1cs_blocked.cuh"], "jubjub.cu": ["mpn_wire.cuh"], "ed25519.cu": ["ed25519.cuh", "mpn_wire.cuh"]}
+EXTRA_DEPS = {"mpn_wire.cu": ["mpn_wire.cuh"], "mpn_host.cu": ["mpn_wire.cuh", "hash_plan.cuh"], "poseidon.cu": ["hash_plan.cuh"], "mpn_prover.cu": ["mpn_wire.cuh"], "mpn_worker.cu": ["mpn_wire.cuh"], "params_io.cu": ["params_io.cuh"], "groth16.cu": ["r1cs_blocked.cuh"], "jubjub.cu": ["mpn_wire.cuh"], "ed25519.cu": ["ed25519.cuh", "mpn_wire.cuh"]}
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -142,6 +142,7 @@ const char *bzk_strerror(int32_t s) {
         case BZK_ERR_UNSAT: return "unsatisfied constraint system";
         case BZK_ERR_BAD_ENCODING: return "bad key file encoding";
         case BZK_ERR_NOT_IN_SUBGROUP: return "point not in the prime-order subgroup";
+        case BZK_ERR_REJECTED: return "proof rejected by its own verifying key";
         default: return "unknown status";
     }
 }

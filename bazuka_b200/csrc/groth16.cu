@@ -667,6 +667,17 @@ int32_t bzk_groth16_params_create(bzk_ctx *ctx, const bzk_g1_affine *alpha_g1, c
     *out = p;
     return BZK_OK;
 }
+int32_t bzk_groth16_params_info(const bzk_groth16_params *p, uint64_t lens[5], bzk_g1_affine *alpha_g1, bzk_g1_affine *beta_g1,
+                                bzk_g2_affine *beta_g2, bzk_g1_affine *delta_g1, bzk_g2_affine *delta_g2) {
+    if (!p) return BZK_ERR_BAD_ARG;
+    if (lens) { lens[0] = p->h->n; lens[1] = p->l->n; lens[2] = p->a->n; lens[3] = p->b1->n; lens[4] = p->b2->n; }
+    if (alpha_g1) to_wire(alpha_g1, p->alpha_g1);
+    if (beta_g1) to_wire(beta_g1, p->beta_g1);
+    if (beta_g2) to_wire(beta_g2, p->beta_g2);
+    if (delta_g1) to_wire(delta_g1, p->delta_g1);
+    if (delta_g2) to_wire(delta_g2, p->delta_g2);
+    return BZK_OK;
+}
 /* frees the handle and the five base vectors it adopted */
 int32_t bzk_groth16_params_free(bzk_ctx *ctx, bzk_groth16_params *p) {
     if (!ctx) return BZK_ERR_BAD_ARG;

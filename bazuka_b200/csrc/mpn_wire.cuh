@@ -195,6 +195,8 @@ bool dec_deposits(const uint8_t *b, size_t n, std::vector<MpnDeposit> &out);
 // bincode of the payment with sig = None: the message its ed25519 signature covers (`ContractDeposit::verify_signature`,
 // src/core/transaction.rs:192-201)
 void enc_contract_deposit_unsigned(Writer &w, const ContractDeposit &p);
+// `bincode::serialize(&MpnConfig)`; false on a truncated image, trailing bytes or a bad tag
+bool dec_config_bytes(const uint8_t *b, size_t n, Config &c);
 
 // sha3-256 (FIPS 202) — `Hasher::hash` of the reference (/root/reference/src/crypto/mod.rs, sha3::Sha3_256)
 void sha3_256(const uint8_t *data, size_t len, uint8_t out[32]);
@@ -257,4 +259,10 @@ int32_t mpn_deposit_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_dep
                                Built<wire::DepositTransition> *out);
 int32_t mpn_withdraw_build_impl(bzk_ctx *ctx, bzk_mpn_state *s, const bzk_mpn_withdraw *wds, uint64_t n_wds, uint32_t log4_batch,
                                 Built<wire::WithdrawTransition> *out);
+// bzk_mpn_prover_prove_work on a decoded work (csrc/mpn_prover.cu); witness_ms (optional): milliseconds until the rows and the
+// witness were done, the context synchronised for it
+int32_t mpn_prover_prove(bzk_ctx *ctx, bzk_mpn_prover *p, const bzk_mpn_work *work, const uint8_t prover_address[32], const bzk_fr *r, const bzk_fr *s,
+                         int32_t check_satisfied, uint8_t zkproof391[391], double *witness_ms);
+// BZK_OK when the key's five vector lengths are those the prover's uploaded R1CS gives (bzk_r1cs_shape), else BZK_ERR_BAD_ARG
+int32_t mpn_prover_key_check(const bzk_mpn_prover *p, const bzk_groth16_params *params);
 }  // namespace bzk

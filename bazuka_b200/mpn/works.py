@@ -325,6 +325,73 @@ class NativeMpnProver:
         self._p = {}
 
 
+class NativeMpnWorker:
+    """the whole worker in libbzk (csrc/mpn_worker.cu): `prove_response(response_bytes, address, seed=None)` ->
+    (PostMpnSolutionRequest bytes, one status per work of the response).  ctxs: the contexts to prove on (several may share a
+    GPU); keys_per_ctx[i]: {"deposit" | "withdraw" | "update": proving key} served on ctxs[i] (a key object with `_h`, or a raw
+    handle) — the update key over the blocked R1CS, deposit and withdraw explicit, each checked at creation against the verifying
+    keys in `config_bytes` (bincode of the node's MpnConfig).  The keys must outlive the worker.  seed (32 bytes) makes the
+    blinding reproducible and is for tests only: without it every proof draws r and s from the OS."""
+
+    KINDS = ("deposit", "withdraw", "update")
+
+    def __init__(self, ctxs, config_bytes, keys_per_ctx, fee_token=ZIESHA):
+        import ctypes as ct
+        import numpy as np
+        from .. import _lib
+        assert len(ctxs) == len(keys_per_ctx) and ctxs
+        self._l, self._ctxs, self._keys = ctxs[0]._l, list(ctxs), [dict(k) for k in keys_per_ctx]
+        handle = lambda k: None if k is None else (k._h if hasattr(k, "_h") else k)
+
+        class Dev(ct.Structure):
+            _fields_ = [("ctx", ct.c_void_p), ("params", ct.c_void_p * 3)]
+        devs = (Dev * len(ctxs))()
+        for i, (c, keys) in enumerate(zip(ctxs, self._keys)):
+            devs[i].ctx = c._h.value if isinstance(c._h, ct.c_void_p) else c._h
+            for k, name in enumerate(self.KINDS):
+                h = handle(keys.get(name))
+                devs[i].params[k] = h.value if isinstance(h, ct.c_void_p) else h
+        canon = lambda v: np.frombuffer((v % N.R).to_bytes(32, "little"), dtype=np.uint64)
+        jj = np.ascontiguousarray(np.stack([canon(N.JJ_D), canon(N.JJ_BASE_COFACTOR[0]), canon(N.JJ_BASE_COFACTOR[1])]))
+        fee = np.ascontiguousarray(canon(fee_token))
+        blob = open(_lib.PARAMS_PATH, "rb").read()
+        cfg = bytes(config_bytes)
+        h = ct.c_void_p()
+        st = self._l.bzk_mpn_worker_create(cfg, len(cfg), ct.byref(devs), len(ctxs), blob, len(blob), ct.c_void_p(jj.ctypes.data),
+                                           ct.c_void_p(fee.ctypes.data), ct.byref(h))
+        if st != 0:
+            raise _lib.BzkError(st, "bzk_mpn_worker_create")
+        self._h = h
+
+    def prove_response(self, response_bytes, address, seed=None):
+        import ctypes as ct
+        import numpy as np
+        from .. import _lib
+        resp = bytes(response_bytes)
+        cap = int.from_bytes(resp[:8], "little") if len(resp) >= 8 else 0
+        status = np.zeros(max(min(cap, 1 << 16), 1), dtype=np.int32)
+        buf, ln, n = ct.c_void_p(), ct.c_size_t(), ct.c_uint64()
+        st = self._l.bzk_mpn_worker_prove_response(self._h, resp, len(resp), bytes(address), None if seed is None else bytes(seed), ct.byref(buf),
+                                                   ct.byref(ln), ct.c_void_p(status.ctypes.data), len(status), ct.byref(n))
+        if st != 0:
+            raise _lib.BzkError(st, "bzk_mpn_worker_prove_response")
+        out = ct.string_at(buf, ln.value)
+        self._l.bzk_buffer_free(buf)
+        return out, [int(x) for x in status[:n.value]]
+
+    def last_timing(self):
+        """{call, rows_witness, prove, self_check} in milliseconds (host clock) of the last prove_response"""
+        import numpy as np
+        ms = np.zeros(4, dtype=np.float64)
+        self._l.bzk_mpn_worker_last_timing(self._h, ms.ctypes.data)
+        return dict(zip(("call", "rows_witness", "prove", "self_check"), (float(x) for x in ms)))
+
+    def free(self):
+        if self._h:
+            self._l.bzk_mpn_worker_free(self._h)
+            self._h = None
+
+
 class WorkerClient:
     """the loop of an MPN worker against a node's HTTP API"""
 
@@ -349,7 +416,14 @@ class WorkerClient:
             self._open("POST", f"http://{self.peer}/bincode/mpn/solution", Wr.post_mpn_solution_request(self.address, proofs)))
 
     def run_once(self, randomness):
-        """fetch the works assigned to this address, prove each, post the proofs; -> (n_works, n_accepted)"""
+        """fetch the works assigned to this address, prove each, post the proofs; -> (n_works, n_accepted).  With a
+        NativeMpnWorker the response goes through one call and the worker draws its own blinding (`randomness` is unused)."""
+        if isinstance(self.prover, NativeMpnWorker):
+            resp = self._open("GET", f"http://{self.peer}/bincode/mpn/work", Wr.get_mpn_work_request(self.address))
+            body, status = self.prover.prove_response(resp, self.address)
+            n_ok = sum(1 for x in status if x == 0)
+            return len(status), (Wr.post_mpn_solution_response_from_bytes(self._open("POST", f"http://{self.peer}/bincode/mpn/solution", body))
+                                 if n_ok else 0)
         works = self.get_works()
         proofs = {}
         for wid, work in works.items():

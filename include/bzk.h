@@ -48,6 +48,7 @@ typedef struct bzk_g2_bases bzk_g2_bases;
 #define BZK_ERR_UNSAT (-7)         /* witness does not satisfy the constraint system */
 #define BZK_ERR_BAD_ENCODING (-8)  /* a key file image is truncated or holds a bad flag, a non-canonical coordinate or a point at infinity */
 #define BZK_ERR_NOT_IN_SUBGROUP (-9) /* a point is on the curve but not in the prime-order subgroup */
+#define BZK_ERR_REJECTED (-10)     /* a proof the prover made failed its own verification (bzk_mpn_worker_prove_response) */
 
 const char *bzk_strerror(int32_t status);
 const char *bzk_last_error(const bzk_ctx *ctx);
@@ -261,6 +262,10 @@ int32_t bzk_groth16_params_create(bzk_ctx *ctx, const bzk_g1_affine *alpha_g1, c
                                   bzk_g1_bases *h, bzk_g1_bases *l, bzk_g1_bases *a, bzk_g1_bases *b_g1, bzk_g2_bases *b_g2,
                                   bzk_groth16_params **out);
 int32_t bzk_groth16_params_free(bzk_ctx *ctx, bzk_groth16_params *params);
+/* What a key handle holds, each output optional: lens = the lengths of its five vectors {h, l, a, b_g1, b_g2} (a shard's: its
+ * slices), and the verifying-key points the proof tail uses, as wire images.  Host only, no device access. */
+int32_t bzk_groth16_params_info(const bzk_groth16_params *params, uint64_t lens[5], bzk_g1_affine *alpha_g1, bzk_g1_affine *beta_g1,
+                                bzk_g2_affine *beta_g2, bzk_g1_affine *delta_g1, bzk_g2_affine *delta_g2);
 /* inputs[num_inputs] (inputs[0] = ONE), aux[num_aux], r, s: host Montgomery images.  With
  * check_satisfied != 0 returns BZK_ERR_UNSAT when a*b != c on some constraint (bellman proves
  * garbage silently).  Outputs are the wire images of Proof {a, b, c}. */
@@ -674,6 +679,51 @@ int32_t bzk_mpn_prover_create(bzk_ctx *ctx, const bzk_mpn_circuit *circuit, cons
 int32_t bzk_mpn_prover_free(bzk_ctx *ctx, bzk_mpn_prover *prover);
 int32_t bzk_mpn_prover_prove_work(bzk_ctx *ctx, bzk_mpn_prover *prover, const uint8_t *work_bytes, size_t work_len, const uint8_t prover_address[32],
                                   const bzk_fr *r, const bzk_fr *s, int32_t check_satisfied, uint8_t zkproof391[391]);
+
+/* ------------------------------------------------------------------ the MPN worker: a node's work response in, the solution out
+ * What a worker does on each poll (the reference's external prover, src/mpn/mod.rs:79-129): `GetMpnWorkResponse` bytes in,
+ * `PostMpnSolutionRequest` bytes out, over one or more contexts, several of them on one GPU if wanted.
+ *   bzk_mpn_worker_create   config = bincode(MpnConfig), the node's; devices[i] = a context and, per kind in MpnWorkData order
+ *                           {deposit, withdraw, update}, that kind's proving key (borrowed, must outlive the worker) or NULL when
+ *                           this context does not serve the kind.  Each served circuit is compiled once at the config's shape
+ *                           (A, T, B of its kind): the update circuit always by the blocked compile, deposit and withdraw
+ *                           explicit; one bzk_mpn_prover per context and kind.  poseidon_blob / jubjub as for the compilers,
+ *                           fee_token canonical (Ziesha = 1).  Every context must have its Poseidon table loaded.
+ *                           BZK_ERR_BAD_ARG: a malformed config, no context, a key whose five vector lengths are not the ones
+ *                           its circuit's R1CS gives (h = m - 1, l = num_aux, a / b_g1 / b_g2 = density counts), or whose
+ *                           alpha_g1, beta_g1, beta_g2, delta_g1 or delta_g2 differ from that kind's verifying key in the config.
+ *   bzk_mpn_worker_prove_response
+ *                           decodes the response (bzk_mpn_get_work_response_decode) and proves every work whose config is the
+ *                           worker's (the same shape and the same verifying-key bytes for its kind), with the satisfiability
+ *                           check on, one host thread per context, largest circuit first.  Before a proof is kept it is checked
+ *                           against the work's verifying key and public inputs (one bzk_groth16_verify_batch per kind).  The proved
+ *                           works are encoded with bzk_mpn_post_solution_request_encode into *solution (release with
+ *                           bzk_buffer_free), in the order of the response.  status_each (optional, one per work on the wire, in
+ *                           response order): BZK_OK proved; BZK_ERR_BAD_ARG a foreign config or a work of a kind no context serves;
+ *                           BZK_ERR_UNSAT transitions that do not satisfy the circuit; BZK_ERR_REJECTED a proof that failed its own
+ *                           verification (the key's point vectors or ic do not belong to the verifying key).  Such works are left
+ *                           out and the call still returns BZK_OK.  A malformed response is BZK_ERR_BAD_ARG with no solution; a
+ *                           device or memory error is returned as such, with no solution.
+ *                           Blinding: seed == NULL draws r and s of every proof from the OS (getrandom, 64 bytes each, reduced mod
+ *                           r).  A non-NULL seed (32 bytes) is a test hook that makes proofs reproducible: r = SHA3(seed || id ||
+ *                           "r"), s = SHA3(seed || id || "s") as little-endian integers mod r, id = the work's u64 id (little-endian)
+ *                           — never use it in production, a predictable r or s gives away the witness.
+ * Each context is driven by one thread of the call at a time; the worker itself launches no kernel of its own. */
+typedef struct bzk_mpn_worker bzk_mpn_worker;
+typedef struct {
+    bzk_ctx *ctx;
+    const bzk_groth16_params *params[3];   /* deposit, withdraw, update; NULL = not served on this context */
+} bzk_mpn_worker_device;
+int32_t bzk_mpn_worker_create(const uint8_t *config_bytes, size_t config_len, const bzk_mpn_worker_device *devices, uint32_t n_devices,
+                              const uint8_t *poseidon_blob, size_t blob_len, const bzk_fr jubjub[3], const bzk_fr *fee_token, bzk_mpn_worker **out);
+int32_t bzk_mpn_worker_prove_response(bzk_mpn_worker *worker, const uint8_t *response, size_t len, const uint8_t prover_address[32],
+                                      const uint8_t *seed32, uint8_t **solution, size_t *solution_len, int32_t *status_each, uint64_t status_cap,
+                                      uint64_t *n_works);
+int32_t bzk_mpn_worker_free(bzk_mpn_worker *worker);
+/* Host wall-clock milliseconds of the last successful prove_response: {the whole call, rows + witness (summed over works, the
+ * context synchronised after each witness), the rest of each proof (summed over works), the self-check}.  With several contexts
+ * the two sums can exceed the call's time. */
+int32_t bzk_mpn_worker_last_timing(const bzk_mpn_worker *worker, double ms[4]);
 
 /* 387-byte bincode image of `Groth16Proof {a,b,c}` (/root/reference/src/zk/groth16/mod.rs:33-38);
  * prefix it with the u32 variant tag 0 for `ZkProof::Groth16` (391 B). */
